@@ -115,6 +115,11 @@ struct Params {
   uint4*    ring;            // 48-B records (3 vectors): n_servers rings of ring_cap_s, then rings of ring_cap
   uint32_t  ring_cap, ring_cap_s;      // per endpoint: others / servers (powers of two)
   uint32_t  n_ep, n_servers, n_inj_tickets, max_window, max_window_s;
+  // broadcast: every server also has a compact ring of ring_cap_s 16-B records {idx, ticket, round_lo, value}
+  // for server -> neighbor gossip, after the 48-B rings in the same allocation (ring + cring_off); its tail /
+  // limit / head are entries cq + e of the arrays above.  cq = 0: no compact rings
+  size_t    cring_off;
+  uint32_t  cq;
   // per-round history (ring of `hist` rows, stride t_max entries)
   RoundMeta* rmeta;
   uint32_t* rt_em;           // emissions per ticket, exclusive prefix once the round is committed

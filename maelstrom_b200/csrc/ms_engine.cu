@@ -621,19 +621,27 @@ static int build_sim(ms_sim* s, const ms_config* in) {
   Params& P = s->P;
   memset(&P, 0, sizeof P);
   const uint32_t M = c.max_endpoints;
+  // broadcast: server -> neighbor gossip travels in 16-B compact records (DESIGN.md 3.1), one more ring per
+  // server behind the 48-B rings, its counters behind the M endpoints' in tail / limit / head
+  const bool compact = c.workload == MS_W_BROADCAST;
+  const size_t n_ctr = (size_t)M + (compact ? c.n_nodes : 0u);
   int rc;
   if ((rc = s->dalloc(&P.st, 1))) return rc;
   if ((rc = s->dalloc(&P.np, 1))) return rc;
   if ((rc = s->dalloc(&P.kind, M))) return rc;
-  if ((rc = s->dalloc(&P.tail, M))) return rc;
-  if ((rc = s->dalloc(&P.limit, M))) return rc;
-  if ((rc = s->dalloc(&P.head, M))) return rc;
+  if ((rc = s->dalloc(&P.tail, n_ctr))) return rc;
+  if ((rc = s->dalloc(&P.limit, n_ctr))) return rc;
+  if ((rc = s->dalloc(&P.head, n_ctr))) return rc;
   if ((rc = s->dalloc(&P.ep_born, M))) return rc;
   {
+    const size_t full_vecs = ((size_t)c.n_nodes * c.server_ring_cap + (size_t)(M - c.n_nodes) * c.ring_cap) * 3;
+    const size_t compact_vecs = compact ? (size_t)c.n_nodes * c.server_ring_cap : 0;
     void* ptr = nullptr;
-    CK(cudaMalloc(&ptr, ((size_t)c.n_nodes * c.server_ring_cap + (size_t)(M - c.n_nodes) * c.ring_cap) * 48));
+    CK(cudaMalloc(&ptr, (full_vecs + compact_vecs) * 16));
     s->allocs.push_back(ptr);
     P.ring = (uint4*)ptr;
+    P.cring_off = full_vecs;
+    P.cq = compact ? M : 0u;
   }
   P.ring_cap = c.ring_cap;
   P.ring_cap_s = c.server_ring_cap;

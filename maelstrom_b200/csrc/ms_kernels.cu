@@ -145,6 +145,45 @@ __device__ __forceinline__ uint4* ring_slot(const Params& p, uint4* ring, uint32
   return ring + (ring_base(p, e) + (pos & (ring_cap_of(p, e) - 1u))) * 3;
 }
 
+// Compact ring of server e (broadcast, p.cq != 0): 16-B records {idx, ticket, round_lo, value} of server ->
+// neighbor gossip.  Everything else of such a message is implied: src = ticket - n_inj_tickets, dest = e,
+// type broadcast without flags, msg_id = in_reply_to = p1 = 0, and the sender's round is the newest round
+// with those low 32 bits that is not after the receiver's (records are consumed the round after they are sent).
+__device__ __forceinline__ uint4* cring_slot(const Params& p, uint4* ring, uint32_t e, uint32_t pos) {
+  return ring + p.cring_off + (size_t)e * p.ring_cap_s + (pos & (p.ring_cap_s - 1u));
+}
+__device__ __forceinline__ uint64_t compact_round(uint64_t round, uint32_t round_lo) {
+  return round - (uint32_t)((uint32_t)round - round_lo);
+}
+
+// The window an endpoint consumes in a round: slots [0, n_full) are 48-B records of its inbox ring from
+// `head` on, slots [n_full, n) compact records of its compact ring from `chead` on.  Only broadcast servers
+// have a compact part, so the other node programs (Raft, txn, services, closed-loop clients) read their
+// 48-B ring directly.
+struct Win {
+  const uint4* ring;
+  const uint4* cring;
+  uint32_t head, chead, mask, n_full;
+};
+// the three vectors of window slot i, as a 48-B record would hold them
+__device__ __forceinline__ void win_load(const Params& p, const Win& w, uint32_t e, uint64_t round, uint32_t i,
+                                         uint4& a, uint4& b, uint4& c) {
+  if (i < w.n_full) {
+    const uint4* rp = w.ring + (size_t)((w.head + i) & w.mask) * 3;
+    a = rp[0]; b = rp[1]; c = rp[2];
+  } else {
+    const uint4 x = w.cring[(w.chead + (i - w.n_full)) & w.mask];
+    a = make_uint4(x.x, x.y, x.z, (uint32_t)(compact_round(round, x.z) >> 32));
+    b = make_uint4(x.y - p.n_inj_tickets, e, 0u, 0u);
+    c = make_uint4((uint32_t)MS_T_BROADCAST, x.w, 0u, 0u);
+  }
+}
+__device__ __forceinline__ Rec win_rec(const Params& p, const Win& w, uint32_t e, uint64_t round, uint32_t i) {
+  uint4 a, b, c;
+  win_load(p, w, e, round, i, a, b, c);
+  return rec_unpack(a, b, c);
+}
+
 // dense id of (round, ticket, idx): id_base[round] + emit_prefix[round][ticket] + idx
 __device__ __forceinline__ uint64_t dense_base(const Params& p, DevState* st, uint64_t round, uint32_t ticket) {
   if (ticket == kResolvedTicket) return round << 32;   // the record already carries its id (k_release)
@@ -561,7 +600,14 @@ __device__ void snapshot_endpoints(const Params& p, DevState* st, uint32_t gid, 
     const uint32_t h = p.limit[e], l = p.tail[e];
     p.head[e] = h;
     p.limit[e] = l;
-    const uint32_t n = ((p.kind[e] & kRemoved)) ? 0u : l - h;
+    uint32_t n = l - h;
+    if (p.cq && e < p.n_servers) {       // the compact ring's window is frozen with the other one
+      const uint32_t ch = p.limit[p.cq + e], cl = p.tail[p.cq + e];
+      p.head[p.cq + e] = ch;
+      p.limit[p.cq + e] = cl;
+      n += cl - ch;
+    }
+    if (p.kind[e] & kRemoved) n = 0;
     // g-set: a node whose periodic replication task is due emits even with an empty window
     // Raft: a node whose election / step-down / replication timers are due acts on an empty window too
     const bool timer_due = e < p.n_servers && p.kind[e] == MS_KIND_SERVER &&
@@ -1464,13 +1510,18 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     const uint32_t e = ticket - p.n_inj_tickets;
     const uint8_t kind = p.kind[e];
     const uint32_t head = p.head[e];
-    uint32_t n = ((kind & kRemoved)) ? 0u : (p.limit[e] - head);
+    const bool has_c = p.cq && e < p.n_servers;
+    const uint32_t chead = has_c ? p.head[p.cq + e] : 0u;
+    uint32_t n_full = p.limit[e] - head;
+    uint32_t n = n_full + (has_c ? p.limit[p.cq + e] - chead : 0u);
+    if (kind & kRemoved) n = n_full = 0;
     if (n > cap || n > (e < p.n_servers ? p.max_window_s : p.max_window)) {
       if (tid == 0) latch_error(st, E_WINDOW_OVERFLOW, e);
-      n = 0;
+      n = n_full = 0;
     }
     const uint4* myring = p.ring + ring_base(p, e) * 3;
     const uint32_t my_mask = ring_cap_of(p, e) - 1u;
+    const Win win{myring, p.ring + p.cring_off + (size_t)e * p.ring_cap_s, head, chead, my_mask, n_full};
     const bool is_server = (kind == MS_KIND_SERVER);
     const bool bcast = !GS && is_server && p.workload == MS_W_BROADCAST;
     // g-set periodic task (g_set.rb:34-39), evaluated before the node's receives: when due, the
@@ -1503,10 +1554,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
 #pragma unroll
         for (int q = 0; q < 2; q++) {
           const int i = base + q * nt + tid;
-          if (i < (int)n) {
-            const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
-            a[q] = rp[0]; b[q] = rp[1]; c[q] = rp[2];
-          }
+          if (i < (int)n) win_load(p, win, e, round, (uint32_t)i, a[q], b[q], c[q]);   // compact slots: one load
         }
 #pragma unroll
         for (int q = 0; q < 2; q++) {
@@ -1609,6 +1657,15 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
           prefetch_l2_bulk(base2 + (size_t)o2 * 3, first * 48u);
           if (n2 > first) prefetch_l2_bulk(base2, (n2 - first) * 48u);
         }
+        if (p.cq && e2 < p.n_servers) {
+          const uint32_t ch2 = p.head[p.cq + e2], nc2 = p.limit[p.cq + e2] - ch2;
+          if (nc2 > 0 && nc2 <= cap2) {
+            const uint4* cbase2 = p.ring + p.cring_off + (size_t)e2 * cap2;
+            const uint32_t o2 = ch2 & (cap2 - 1u), first = min(nc2, cap2 - o2);
+            prefetch_l2_bulk(cbase2 + o2, first * 16u);
+            if (nc2 > first) prefetch_l2_bulk(cbase2, (nc2 - first) * 16u);
+          }
+        }
       }
     }
 
@@ -1620,8 +1677,10 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     uint32_t R = 0;
     bool use_blocks = false;
     if (n > 0) {
-      // block starts: each thread scans one contiguous segment of the window
+      // block starts: each thread scans one contiguous segment of the window; the compact part of the
+      // window (from slot n_full on) always starts a block of its own
       const int c = ((int)n + nt - 1) / nt;
+      const int nfull = (int)n_full;
       const int lo = min(tid * c, (int)n), hi = min(lo + c, (int)n);
       uint32_t nf = 0;
       uint32_t fmask = 0;                       // block starts of this thread's segment (when it has <= 32 slots)
@@ -1632,7 +1691,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         for (int i = lo; i < hi; i++) {
           const uint64_t ka = keyA[i];
           const uint32_t kb = keyB[i];
-          if (i == 0 || ka != pa || kb <= pb) { nf++; fmask |= 1u << ((i - lo) & 31); }
+          if (i == 0 || i == nfull || ka != pa || kb <= pb) { nf++; fmask |= 1u << ((i - lo) & 31); }
           pa = ka; pb = kb;
         }
       }
@@ -1642,7 +1701,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
           while (fmask) { s_bstart[off++] = (uint16_t)(lo + __ffs(fmask) - 1); fmask &= fmask - 1u; }
         } else {
           for (int i = lo; i < hi; i++)
-            if (i == 0 || keyA[i] != keyA[i - 1] || keyB[i] <= keyB[i - 1]) s_bstart[off++] = (uint16_t)i;
+            if (i == 0 || i == nfull || keyA[i] != keyA[i - 1] || keyB[i] <= keyB[i - 1]) s_bstart[off++] = (uint16_t)i;
         }
         if (tid == 0) s_bstart[R] = (uint16_t)n;
         __syncthreads();
@@ -2000,6 +2059,8 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     const bool agg_ok = nb_smem && n_new > 0 && !need_rng && const_lat == 0 && s_misc[3] == 0;
     const int agg_mode = !agg_ok ? 0 : (use_blocks ? 1 : (deg <= 4 ? 2 : 0));
     const bool agg = agg_mode != 0;
+    // ... and with no endpoint removed that gossip travels as 16-B compact records (PE2's fast path)
+    const bool compact = agg && !np.any_removed && p.cq != 0;
     uint32_t* F01 = keyB;                                   // mode 2: new-from-neighbor 0/1 before pos (2 x u16)
     uint32_t* F23 = reinterpret_cast<uint32_t*>(tab);       //         new-from-neighbor 2/3 before pos
     uint64_t f_total = 0;
@@ -2050,8 +2111,9 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       uint32_t base = 0;
       if (total) {
         const uint32_t o = owner_of(nb, p.n_servers, p.n_shards);
-        base = atomicAdd(&p.tail_sh[o][nb], total);
-        if ((uint32_t)(base + total - p.head_sh[o][nb]) > ring_cap_of(p, nb)) latch_error(st, E_RING_OVERFLOW, nb);
+        const uint32_t ci = compact ? p.cq + nb : nb;      // the compact ring's counters, or the 48-B ring's
+        base = atomicAdd(&p.tail_sh[o][ci], total);
+        if ((uint32_t)(base + total - p.head_sh[o][ci]) > ring_cap_of(p, nb)) latch_error(st, E_RING_OVERFLOW, nb);
       }
       s_nbbase[tid] = base;
     }
@@ -2078,8 +2140,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       const uint32_t mt = meta[i];
       const uint32_t sslot = mt & M_SRCSLOT;
       if (full_recv || !nb_smem || sslot == 0) {
-        const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
-        Rec m = rec_unpack(rp[0], rp[1], rp[2]);
+        Rec m = win_rec(p, win, e, round, i);
         const uint64_t id = (use_blocks ? s_bbase[blk[pos]] : dense_base(p, st, m.round, m.ticket)) + m.idx;
         journal_raw(p, cx.chunk + k, id, true, m);
         const bool cl = cl_ep || (m.src >= p.n_servers && kind_is_client(p.kind[m.src]));
@@ -2182,10 +2243,10 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
             direct = s_nbbase[js] + new_before - (f & 0xFFFFu);
             has_direct = true;
           }
-          fast = has_direct && !np.any_removed;
+          fast = compact;
         } else {
-          const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
-          const uint4 vb = rp[1], vc = rp[2];
+          uint4 va, vb, vc;
+          win_load(p, win, e, round, i, va, vb, vc);
           MsgView w;
           w.src = vb.x; w.msg_id = vb.z; w.tf = vc.x; w.p0 = vc.y;
           const uint64_t p1 = (uint64_t)vc.z | ((uint64_t)vc.w << 32);
@@ -2217,14 +2278,14 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         }
       }
       if (fast) {
-        // server -> neighbor gossip into ring space this CTA already claimed: what emit_one does for it, without
-        // the general case's lookups (both ends are live servers, zero constant latency, no loss: agg_ok)
+        // server -> neighbor gossip into compact ring space this CTA already claimed: what emit_one does for it,
+        // without the general case's lookups (both ends are live servers, zero constant latency, no loss: agg_ok)
         r.round = round; r.ticket = ticket; r.idx = j;                         // order key == id order (net.clj:197)
         journal_raw(p, cx.chunk + n_recv + j, j, false, r);                    // net.clj:208
         cx.c_send_sv++;
         cx.c_zero++;
         uint4* ring_o = p.ring_sh[owner_of(r.dest, p.n_servers, p.n_shards)];
-        rec_store(ring_o + ((size_t)r.dest * p.ring_cap_s + (direct & (p.ring_cap_s - 1u))) * 3, r);
+        st_v4(cring_slot(p, ring_o, r.dest, direct), make_uint4(j, ticket, (uint32_t)round, r.p0));
       }
       if (__any_sync(FULL, valid && !fast)) emit_one(p, st, np, cx, valid && !fast, r, j, direct, has_direct);
     }
