@@ -367,6 +367,13 @@ int      ms_raft_state(ms_sim* sim, uint32_t node, uint64_t out[8]);
  * kernel launches, lost, partition_drops, max_window, windows that needed the full sort} */
 int ms_counters(ms_sim* sim, uint64_t out[8]);
 
+/* inbox ring occupancy of the servers (n_nodes = S), as the last round left it: out = six arrays of S
+ * entries {tail, limit, head} of the 48-B ring, then {tail, limit, head} of the 16-B compact gossip ring
+ * (broadcast only, zero otherwise).  tail counts claimed records, [head, limit) is the window the
+ * last snapshot froze, tail - limit records are still pending.  The counters are 32-bit and wrap;
+ * servers another shard owns read 0.  n = capacity of out in entries (>= 6 S); returns S. */
+int ms_ring_counters(ms_sim* sim, uint64_t* out, uint32_t n);
+
 /* ------------------------------------------------------------------ multi-GPU (one process per GPU)
  * Endpoints are sharded by index range; every shard runs the same rounds in lock step.
  * A message for an endpoint of another shard is written by the sending kernel straight

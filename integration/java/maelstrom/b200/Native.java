@@ -55,6 +55,7 @@ public final class Native {
   public static native long undeliverable(long h);
   public static native int raftState(long h, int node, ByteBuffer out8);
   public static native int counters(long h, ByteBuffer out8);
+  public static native int ringCounters(long h, ByteBuffer out, int n);
   public static native int shardHandles(long h, ByteBuffer blob512);
   public static native int shardConnect(long h, int peer, ByteBuffer blob512);
   public static native int setBarrierDefault(long h);

@@ -112,6 +112,7 @@ SYMBOLS = {
     "ms_undeliverable": (C.c_uint64, [_P]),
     "ms_raft_state": (C.c_int, [_P, C.c_uint32, _P]),
     "ms_counters": (C.c_int, [_P, _P]),
+    "ms_ring_counters": (C.c_int, [_P, _P, C.c_uint32]),
     "ms_timer_begin": (C.c_int, [_P]),
     "ms_timer_end": (C.c_int, [_P, C.POINTER(C.c_double)]),
     "ms_profile": (C.c_int, [_P, C.c_int]),

@@ -367,4 +367,10 @@ MS_HD uint32_t owner_of_ticket(uint32_t t, uint32_t n_inj, uint32_t n_servers, u
   return t < n_inj ? 0u : owner_of(t - n_inj, n_servers, G);
 }
 
+// The sender's 64-bit round of a compact gossip record, which keeps only its low 32 bits: the newest
+// round with those low bits that is not after the receiver's `round`.
+MS_HD uint64_t compact_round(uint64_t round, uint32_t round_lo) {
+  return round - (uint32_t)((uint32_t)round - round_lo);
+}
+
 }  // namespace msd

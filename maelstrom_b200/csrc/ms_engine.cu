@@ -1879,6 +1879,29 @@ int ms_counters(ms_sim* s, uint64_t out[8]) {
   return MS_OK;
 }
 
+int ms_ring_counters(ms_sim* s, uint64_t* out, uint32_t n) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  const uint32_t S = s->P.n_servers;
+  if (!out || n < 6u * S) { set_err("ms_ring_counters: out needs 6 x n_nodes entries"); return MS_ERR_ARG; }
+  std::vector<uint32_t> t(S), l(S), h(S);
+  memset(out, 0, (size_t)6 * S * sizeof(uint64_t));
+  CK(cudaStreamSynchronize(s->stream));
+  for (uint32_t part = 0; part < 2; part++) {
+    if (part == 1 && !s->P.cq) break;                  // no compact rings: that half stays zero
+    const size_t off = part ? s->P.cq : 0u;
+    CK(cudaMemcpy(t.data(), s->P.tail + off, S * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(l.data(), s->P.limit + off, S * 4, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(h.data(), s->P.head + off, S * 4, cudaMemcpyDeviceToHost));
+    uint64_t* o = out + (size_t)part * 3 * S;
+    for (uint32_t e = 0; e < S; e++) {
+      if (owner_of(e, S, s->P.n_shards) != s->P.shard_id) continue;   // another shard's server: its counters live there
+      o[e] = t[e]; o[S + e] = l[e]; o[2 * S + e] = h[e];
+    }
+  }
+  return (int)S;
+}
+
 struct ShardBlob {   // MS_SHARD_BLOB_BYTES
   uint32_t magic, shard_id, n_shards, t_max;
   uint32_t max_endpoints, ring_cap, hist, pad;

@@ -187,6 +187,8 @@ jlong FN(clientReplies)(JNIEnv* env, jclass c, jlong h) { (void)env; (void)c; re
 jlong FN(undeliverable)(JNIEnv* env, jclass c, jlong h) { (void)env; (void)c; return (jlong)ms_undeliverable(H(h)); }
 jint FN(raftState)(JNIEnv* env, jclass c, jlong h, jint node, jobject out8) { (void)c; return ms_raft_state(H(h), (uint32_t)node, (uint64_t*)BUF(out8)); }
 jint FN(counters)(JNIEnv* env, jclass c, jlong h, jobject out8) { (void)c; return ms_counters(H(h), (uint64_t*)BUF(out8)); }
+/* out = direct buffer of n u64 (>= 6 x n_nodes): tail / limit / head of the 48-B rings, then of the compact rings */
+jint FN(ringCounters)(JNIEnv* env, jclass c, jlong h, jobject out, jint n) { (void)c; return ms_ring_counters(H(h), (uint64_t*)BUF(out), (uint32_t)n); }
 
 /* multi-GPU plumbing (one JVM per GPU, or one JVM driving several handles) */
 jint FN(shardHandles)(JNIEnv* env, jclass c, jlong h, jobject blob) { (void)c; return ms_shard_handles(H(h), BUF(blob)); }

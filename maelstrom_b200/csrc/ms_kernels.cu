@@ -148,12 +148,10 @@ __device__ __forceinline__ uint4* ring_slot(const Params& p, uint4* ring, uint32
 // Compact ring of server e (broadcast, p.cq != 0): 16-B records {idx, ticket, round_lo, value} of server ->
 // neighbor gossip.  Everything else of such a message is implied: src = ticket - n_inj_tickets, dest = e,
 // type broadcast without flags, msg_id = in_reply_to = p1 = 0, and the sender's round is the newest round
-// with those low 32 bits that is not after the receiver's (records are consumed the round after they are sent).
+// with those low 32 bits that is not after the receiver's (compact_round in ms_device.cuh; records are consumed
+// the round after they are sent).
 __device__ __forceinline__ uint4* cring_slot(const Params& p, uint4* ring, uint32_t e, uint32_t pos) {
   return ring + p.cring_off + (size_t)e * p.ring_cap_s + (pos & (p.ring_cap_s - 1u));
-}
-__device__ __forceinline__ uint64_t compact_round(uint64_t round, uint32_t round_lo) {
-  return round - (uint32_t)((uint32_t)round - round_lo);
 }
 
 // The window an endpoint consumes in a round: slots [0, n_full) are 48-B records of its inbox ring from

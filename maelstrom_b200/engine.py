@@ -321,6 +321,17 @@ class Sim:
         names = ("rounds", "sends", "recvs", "launches", "lost", "partition_drops", "max_window", "fallback_sorts")
         return {k: int(v) for k, v in zip(names, out)}
 
+    RING_FIELDS = ("tail", "limit", "head", "ctail", "climit", "chead")
+
+    def ring_counters(self):
+        """ms_ring_counters: per-server uint32 arrays (index = server) of the 48-B inbox ring's tail / limit /
+        head and the compact gossip ring's (ctail / climit / chead; zero without compact rings).  They wrap
+        at 2^32: take differences modulo 2^32.  Servers of other shards read 0."""
+        S = self.n_nodes
+        out = np.zeros(6 * S, dtype=np.uint64)
+        self._chk(self.L.ms_ring_counters(self.h, out.ctypes.data, out.size))
+        return {k: out[i * S:(i + 1) * S].astype(np.uint32) for i, k in enumerate(self.RING_FIELDS)}
+
     def timer_begin(self):
         return self._chk(self.L.ms_timer_begin(self.h))
 

@@ -17,6 +17,7 @@ uint64_t dm_latency(uint32_t dist, uint32_t mean_ms, uint32_t scale, uint64_t ex
   return msd::latency_ms(np, x);
 }
 uint32_t dm_owner(uint32_t e, uint32_t n_servers, uint32_t g) { return msd::owner_of(e, n_servers, g); }
+uint64_t dm_compact_round(uint64_t round, uint32_t round_lo) { return msd::compact_round(round, round_lo); }
 uint32_t dm_sizeof_devstate(void) { return (uint32_t)sizeof(msd::DevState); }
 uint32_t dm_sizeof_roundmeta(void) { return (uint32_t)sizeof(msd::RoundMeta); }
 }

@@ -47,6 +47,26 @@ def assert_same_journal(g, o):
     return ev_g, bd_g
 
 
+def oracle_gossip_sends(ev, bd, n_nodes):
+    """Server -> server broadcast gossip in an oracle journal (level 2: events and bodies): the :send events
+    with src and dest < n_nodes, type broadcast and no reply flag.  These are the messages the engine may
+    carry as 16-B compact records."""
+    send = (ev["event_id"] & np.uint64(O.RECV_BIT)) == 0
+    gossip = (send & (ev["src"] < n_nodes) & (ev["dest"] < n_nodes) & (bd["type"] == O.T["broadcast"]) &
+              ((bd["flags"] & O.F_REPLY) == 0))
+    return int(np.count_nonzero(gossip))
+
+
+def compact_total(rc):
+    """Records claimed on all compact rings so far (Sim.ring_counters(); counters start at 0 and wrap)."""
+    return int(rc["ctail"].astype(np.uint64).sum())
+
+
+def compact_delta(rc1, rc0):
+    """Compact records claimed between two ring_counters() reads, per server (modulo 2^32)."""
+    return (rc1["ctail"] - rc0["ctail"]).astype(np.uint32)
+
+
 def ops_array(rows):
     """rows: (time_ns, src, dest, type, msg_id, p0)"""
     a = np.zeros(len(rows), dtype=O.OP_DTYPE)

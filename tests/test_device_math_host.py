@@ -26,6 +26,8 @@ def dm(tmp_path_factory):
     L.dm_latency.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64, C.c_void_p]
     L.dm_owner.restype = C.c_uint32
     L.dm_owner.argtypes = [C.c_uint32, C.c_uint32, C.c_uint32]
+    L.dm_compact_round.restype = C.c_uint64
+    L.dm_compact_round.argtypes = [C.c_uint64, C.c_uint32]
     return L
 
 
@@ -74,6 +76,39 @@ def test_engine_owner_function(dm):
             assert owners[:n_servers] == sorted(owners[:n_servers]) and max(owners) == (g - 1 if n_servers >= g else max(owners))
             counts = np.bincount(owners[:n_servers], minlength=g)
             assert counts.max() - counts.min() <= 1
+
+
+def test_compact_round_rebuilds_the_sender_round(dm):
+    # a compact gossip record keeps the low 32 bits of its sender's round; the receiver (at round R, the sender's
+    # round + d) rebuilds the 64-bit round.  No simulation reaches round 2^32, so this is the only check there.
+    rng = np.random.default_rng(11)
+    receivers = [r for c in (2 ** 32, 2 ** 33, 5 * 2 ** 32) for r in range(c - 4, c + 5)]
+    receivers += [int(x) for x in rng.integers(0, 2 ** 40, 200)] + [0, 1, 2 ** 40 - 1]
+    for R in receivers:
+        for d in (0, 1, 2, 3, 7, 64, 2 ** 16, 2 ** 31, 2 ** 32 - 1):
+            s = R - d
+            if s < 0:
+                continue
+            assert dm.dm_compact_round(R, s & 0xFFFFFFFF) == s, (R, d)
+    # the newest round with those low bits that is not after R: never a later round, never 2^32 too early
+    for R in (2 ** 32 - 1, 2 ** 32, 2 ** 32 + 1):
+        for lo in (0, 1, 0xFFFFFFFE, 0xFFFFFFFF, R & 0xFFFFFFFF):
+            got = dm.dm_compact_round(R, lo)
+            assert got <= R and R - got < 2 ** 32 and got & 0xFFFFFFFF == lo, (R, lo, got)
+
+
+def test_compact_order_key_is_monotone_across_2_32(dm):
+    # k_round orders a window by (round << 24) | ticket with the round a compact slot rebuilds: consecutive
+    # sender rounds across the 2^32 boundary (each read one round later) must give increasing keys
+    for c in (2 ** 32, 2 ** 33, 2 ** 39):
+        keys = []
+        for s in range(c - 3, c + 4):
+            rebuilt = dm.dm_compact_round(s + 1, s & 0xFFFFFFFF)
+            assert rebuilt == s
+            for ticket in (8, 9, 0xFFFFFF):
+                keys.append(((rebuilt << 24) | ticket) & (2 ** 64 - 1))
+        assert keys == sorted(keys) and len(set(keys)) == len(keys)
+        assert keys[-1] == ((c + 3) << 24) | 0xFFFFFF          # no bit of the round lost to the 64-bit key
 
 
 def test_bench_numpy_philox_matches_oracle():

@@ -302,6 +302,53 @@ def test_emulated_shards_discarded_journal_adaptive_batches():
     assert st["servers"]["recv-count"] > 5000
 
 
+@pytest.mark.parametrize("glue", [True, False], ids=["glue", "no_glue"])
+@pytest.mark.parametrize("world", [2, 3, 4])
+def test_emulated_shards_claim_peer_compact_rings(world, glue, monkeypatch):
+    # an 8 x 8 grid whose rows are split across the shards: gossip over a row boundary claims compact ring space
+    # on a peer shard.  Every shard reports its own servers' ring counters; together they must be the single-shard
+    # run's, and the compact records the oracle's server -> server broadcast sends.  MS_NO_GLUE=1 takes the
+    # k_snapshot launch instead of k_glue between rounds.
+    from maelstrom_b200.sharded import shard_owner
+    from scenarios import compact_total, oracle_gossip_sends
+    if not glue:
+        monkeypatch.setenv("MS_NO_GLUE", "1")
+    n = 64
+    kw = dict(topology="grid", n_values=1024, seed=29)
+    counters = {}
+    lock = threading.Lock()
+
+    def scenario(s, body):
+        cs = [s.add_endpoint("c%d" % i, O.KIND_SIM_CLIENT) for i in range(3)]
+        ops, _ = random_broadcast_ops(n, cs, n_ticks=6, per_tick=20, seed=33)
+        s.schedule(ops)
+        s.run(3_000_000)
+        s.run(12_000_000)
+        if hasattr(s, "ring_counters") and s.cfg.n_shards > 1:
+            with lock:
+                counters[s.cfg.shard_id] = s.ring_counters()
+
+    sim_kw = dict(workload="broadcast", ring_cap=1024, max_window=512, journal_cap_log2=19, max_endpoints=n + 8, **kw)
+    ev, st, now, rnd = run_sharded_scenario(world, n, sim_kw, scenario)
+    o = O.Sim(n, workload=O.W_BROADCAST, **kw)
+    check_against_oracle(o, scenario, ev, st, now, rnd)
+    ev_o, bd_o = o.journal()
+    from maelstrom_b200.engine import Sim
+    with emul_lib.use():
+        one = Sim(n, journal_level=1, **sim_kw)
+        scenario(one, None)
+        single = one.ring_counters()
+        one.close()
+    owners = np.array([shard_owner(e, n, world) for e in range(n)])
+    assert len(set(owners.tolist())) == world
+    for k, v in single.items():
+        summed = sum(counters[r][k].astype(np.uint64) for r in range(world))
+        assert np.array_equal(summed, v.astype(np.uint64)), k
+        for r in range(world):                          # a shard reports only the servers it owns
+            assert not counters[r][k][owners != r].any(), (k, r)
+    assert compact_total(single) == oracle_gossip_sends(ev_o, bd_o, n) > 1000
+
+
 def test_emulated_eight_shards_broadcast_glue_path():
     # the shard count of the driver's scaling run: 8 shards, no timing wheel -> one k_glue launch between rounds
     world, n = 8, 64

@@ -11,7 +11,7 @@ import contextlib
 
 import emul_lib
 import oracle_lib as O
-from scenarios import assert_same_journal, both, make_pair
+from scenarios import assert_same_journal, both, compact_total, make_pair, oracle_gossip_sends
 
 
 def backend():
@@ -20,6 +20,31 @@ def backend():
     if os.environ.get("MS_FUZZ_BACKEND") == "cuda":
         return contextlib.nullcontext()
     return emul_lib.use()
+
+
+def compact_expectation(workload, topology, latency_mean_ms, p_loss, loss_phase=False):
+    """How much server -> server gossip a drawn scenario must carry in compact records (DESIGN.md 3.1):
+    "eq" all of it, "le" at most all of it, "zero" none.  The fast path needs broadcast, constant latency 0,
+    no loss roll, no removed endpoint, no message sent on a server's behalf (the fuzzer sends none of these
+    two) and at most 4 neighbors for windows that are not block-ordered."""
+    if workload != "broadcast" or topology == "total" or latency_mean_ms > 0:
+        return "zero"
+    if p_loss > 0 or loss_phase or topology == "tree4":
+        return "le"
+    return "eq"
+
+
+def assert_gossip_accounting(rings, o, expect):
+    """rings: Sim.ring_counters() of every shard; o: the oracle after the same scenario."""
+    ev, bd = o.journal()
+    want = oracle_gossip_sends(ev, bd, o.n_nodes)
+    got = sum(compact_total(rc) for rc in rings)
+    if expect == "eq":
+        assert got == want, (got, want)
+    elif expect == "le":
+        assert got <= want, (got, want)
+    else:
+        assert got == 0, got
 
 
 def seeds():
@@ -155,6 +180,8 @@ def test_random_scenario(seed):
         g, o = make_pair(n, workload=workload, **kw, **sizing)
         rg, ro = both(g, o, scenario)
         assert rg == ro
+        loss_phase = any(fault == 5 and int(fault_args[ph][0]) % 40 for ph, (fault, _, _) in enumerate(plan))
+        assert_gossip_accounting([g.ring_counters()], o, compact_expectation(workload, topo, mean, kw["p_loss"], loss_phase))
         assert_same_journal(g, o)
 
 
@@ -212,6 +239,7 @@ def test_random_heavy_broadcast(seed):
             if "max_window" in str(e) or "ring overflow" in str(e) or "timing wheel" in str(e):
                 pytest.skip("capacity: %s" % e)
             raise
+        assert_gossip_accounting([g.ring_counters()], o, compact_expectation("broadcast", topo, mean, kw["p_loss"]))
         if sizing["journal_level"] == 2:
             assert_same_journal(g, o)
         else:
@@ -248,6 +276,7 @@ def test_random_sharded(seed):
         kw["gset_interval_ms"] = int(rng.integers(4, 12))
     n_clients = int(rng.integers(1, 5))
     ticks, per_tick = int(rng.integers(3, 10)), int(rng.integers(5, 60))
+    rings = {}
 
     def scenario(s, body):
         services = {}
@@ -261,13 +290,18 @@ def test_random_sharded(seed):
         r2 = np.random.default_rng(seed)
         s.schedule(random_ops(r2, n, clients, services, workload, 0, ticks, per_tick, [0] * n_clients))
         s.run((ticks + 30 + 12 * mean) * 1_000_000)
+        if hasattr(s, "ring_counters"):
+            rings[s.cfg.shard_id] = s.ring_counters()     # (one entry per shard thread)
 
     rng_services = bool(rng.integers(2))
     wl = {"broadcast": O.W_BROADCAST, "g-set": O.W_GSET, "txn-list-append": O.W_TXN}[workload]
     ev, st, now, rnd = run_sharded_scenario(
         world, n, dict(workload=workload, ring_cap=2048, max_window=1024, journal_cap_log2=20, max_endpoints=n + 24,
                        calendar_slots=256, calendar_cap=8192, **kw), scenario)
-    check_against_oracle(O.Sim(n, workload=wl, **kw), scenario, ev, st, now, rnd)
+    o = O.Sim(n, workload=wl, **kw)
+    check_against_oracle(o, scenario, ev, st, now, rnd)
+    assert len(rings) == world
+    assert_gossip_accounting(list(rings.values()), o, compact_expectation(workload, kw["topology"], mean, kw["p_loss"]))
 
 
 def raft_seeds():

@@ -43,6 +43,8 @@ def _worker(rank, world, port, q, n, per_tick, latency_ms):
         g.run(40_000_000 if latency_ms else 4_000_000)
         ev = g.gather_journal()
         st = g.stats()
+        rings = [None] * world
+        dist.all_gather_object(rings, g.ring_counters())
         if rank == 0:
             o = O.Sim(n, workload=O.W_BROADCAST, topology="grid", n_values=4 * per_tick + 8,
                       latency_dist="constant", latency_mean_ms=latency_ms)
@@ -56,6 +58,14 @@ def _worker(rank, world, port, q, n, per_tick, latency_ms):
                 assert np.array_equal(ev[f], ev_o[f]), f
             assert st == o.stats()
             assert g.now == o.now and g.round == o.round
+            # gossip across the row split claims compact ring space on the peer GPU: every shard reports its
+            # own servers, together all server -> server broadcast sends (latency 0) or none (latency > 0)
+            from scenarios import compact_total, oracle_gossip_sends
+            got = sum(compact_total(rc) for rc in rings)
+            ev_o, bd_o = o.journal()
+            assert got == (oracle_gossip_sends(ev_o, bd_o, n) if latency_ms == 0 else 0), got
+            if latency_ms == 0:
+                assert got > 0
         q.put((rank, "ok"))
     except Exception:   # noqa: BLE001
         q.put((rank, "FAIL: " + traceback.format_exc()))
