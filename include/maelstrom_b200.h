@@ -374,6 +374,16 @@ int ms_counters(ms_sim* sim, uint64_t out[8]);
  * servers another shard owns read 0.  n = capacity of out in entries (>= 6 S); returns S. */
 int ms_ring_counters(ms_sim* sim, uint64_t* out, uint32_t n);
 
+/* Start a fresh simulation as if `round` rounds, `msg_id` messages and `event_id` journal events had
+ * already happened, with the inbox counters (tail / limit / head, both ring parts) of endpoint e at
+ * ring_pos + e * ring_stride (mod 2^32).  For testing the engine across the 32-bit boundaries of its
+ * counters.  Virtual time stays 0, journal positions stay 0-based (event ids become event_id + position).
+ * Valid only before the first send, schedule or round; endpoints may exist already.  Rejects
+ * round >= 2^39 (the (round << 24) | ticket order key) and msg_id or event_id >= 2^62 with MS_ERR_ARG.
+ * Sharded runs: call it on every shard with the same arguments; each sets its own endpoints. */
+int ms_set_origin(ms_sim* sim, uint64_t round, uint64_t msg_id, uint64_t event_id, uint32_t ring_pos,
+                  uint32_t ring_stride);
+
 /* ------------------------------------------------------------------ multi-GPU (one process per GPU)
  * Endpoints are sharded by index range; every shard runs the same rounds in lock step.
  * A message for an endpoint of another shard is written by the sending kernel straight

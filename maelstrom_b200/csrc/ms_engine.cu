@@ -1902,6 +1902,54 @@ int ms_ring_counters(ms_sim* s, uint64_t* out, uint32_t n) {
   return (int)S;
 }
 
+int ms_set_origin(ms_sim* s, uint64_t round, uint64_t msg_id, uint64_t event_id, uint32_t ring_pos, uint32_t ring_stride) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  if (round >= (1ull << 39) || msg_id >= (1ull << 62) || event_id >= (1ull << 62)) {
+    set_err("ms_set_origin: round must be < 2^39 (order keys), msg_id and event_id < 2^62");
+    return MS_ERR_ARG;
+  }
+  if (s->hs.rounds_run || !s->pending.empty() || !s->sched.empty()) {
+    set_err("ms_set_origin: only a fresh simulation (no send, schedule or round yet) can be moved");
+    return MS_ERR_ARG;
+  }
+  Params& P = s->P;
+  CK(cudaStreamSynchronize(s->stream));
+  s->hs.round = round;
+  s->hs.drain_round = round;
+  s->hs.next_id = msg_id;
+  s->hs.next_event = event_id;
+  s->hs.journal_drained = event_id;
+  CK(cudaMemcpy(P.st, &s->hs, sizeof(DevState), cudaMemcpyHostToDevice));
+  // the round history as build_sim leaves it, opened at `round` instead of 0
+  std::vector<RoundMeta> rows(P.hist);
+  memset(rows.data(), 0, rows.size() * sizeof(RoundMeta));
+  for (RoundMeta& m : rows) m.round = ~0ull;
+  RoundMeta& r0 = rows[(size_t)(round & P.hist_mask)];
+  r0.round = round;
+  r0.now = s->hs.now;
+  r0.id_base = msg_id;
+  r0.ev_base = event_id;
+  r0.raw_base = s->hs.jraw_cursor;
+  CK(cudaMemcpy(P.rmeta, rows.data(), rows.size() * sizeof(RoundMeta), cudaMemcpyHostToDevice));
+  // no message has an id below the origin: every endpoint slot counts as born there
+  const uint32_t M = s->cfg.max_endpoints;
+  std::vector<uint64_t> born(M, msg_id);
+  CK(cudaMemcpy(P.ep_born, born.data(), (size_t)M * 8, cudaMemcpyHostToDevice));
+  // ring counters of this shard's endpoints: the 48-B part for every endpoint, the compact part for the servers
+  const size_t n_ctr = (size_t)M + (P.cq ? P.n_servers : 0u);
+  std::vector<uint32_t> ctr(n_ctr);
+  CK(cudaMemcpy(ctr.data(), P.tail, n_ctr * 4, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n_ctr; i++) {
+    const uint32_t e = i < M ? (uint32_t)i : (uint32_t)(i - P.cq);
+    if (owner_of(e, P.n_servers, P.n_shards) == P.shard_id) ctr[i] = ring_pos + e * ring_stride;
+  }
+  CK(cudaMemcpy(P.tail, ctr.data(), n_ctr * 4, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(P.limit, ctr.data(), n_ctr * 4, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(P.head, ctr.data(), n_ctr * 4, cudaMemcpyHostToDevice));
+  return MS_OK;
+}
+
 struct ShardBlob {   // MS_SHARD_BLOB_BYTES
   uint32_t magic, shard_id, n_shards, t_max;
   uint32_t max_endpoints, ring_cap, hist, pad;

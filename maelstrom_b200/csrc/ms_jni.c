@@ -189,6 +189,11 @@ jint FN(raftState)(JNIEnv* env, jclass c, jlong h, jint node, jobject out8) { (v
 jint FN(counters)(JNIEnv* env, jclass c, jlong h, jobject out8) { (void)c; return ms_counters(H(h), (uint64_t*)BUF(out8)); }
 /* out = direct buffer of n u64 (>= 6 x n_nodes): tail / limit / head of the 48-B rings, then of the compact rings */
 jint FN(ringCounters)(JNIEnv* env, jclass c, jlong h, jobject out, jint n) { (void)c; return ms_ring_counters(H(h), (uint64_t*)BUF(out), (uint32_t)n); }
+/* test origin of a fresh simulation: round, message id, event id, ring counters ring_pos + e * ring_stride */
+jint FN(setOrigin)(JNIEnv* env, jclass c, jlong h, jlong round, jlong msg_id, jlong event_id, jint ring_pos, jint ring_stride) {
+  (void)env; (void)c;
+  return ms_set_origin(H(h), (uint64_t)round, (uint64_t)msg_id, (uint64_t)event_id, (uint32_t)ring_pos, (uint32_t)ring_stride);
+}
 
 /* multi-GPU plumbing (one JVM per GPU, or one JVM driving several handles) */
 jint FN(shardHandles)(JNIEnv* env, jclass c, jlong h, jobject blob) { (void)c; return ms_shard_handles(H(h), BUF(blob)); }

@@ -332,6 +332,13 @@ class Sim:
         self._chk(self.L.ms_ring_counters(self.h, out.ctypes.data, out.size))
         return {k: out[i * S:(i + 1) * S].astype(np.uint32) for i, k in enumerate(self.RING_FIELDS)}
 
+    def set_origin(self, round=0, msg_id=0, event_id=0, ring_pos=0, ring_stride=0):
+        """ms_set_origin: start this fresh simulation as if `round` rounds, `msg_id` messages and `event_id`
+        events had happened, with endpoint e's inbox counters at ring_pos + e * ring_stride (mod 2^32).
+        For tests at the 32-bit boundaries of the engine's counters; only before any send, schedule or round."""
+        return self._chk(self.L.ms_set_origin(self.h, round, msg_id, event_id, ring_pos & 0xFFFFFFFF,
+                                              ring_stride & 0xFFFFFFFF))
+
     def timer_begin(self):
         return self._chk(self.L.ms_timer_begin(self.h))
 

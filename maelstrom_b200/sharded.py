@@ -83,6 +83,11 @@ class ShardedSim:
     def __getattr__(self, name):                      # add_endpoint, schedule, run, step, ...
         return getattr(self.sim, name)
 
+    def set_origin(self, *args, **kw):
+        """ms_set_origin on this rank's shard; every rank calls it with the same arguments (each shard sets its
+        own endpoints' ring counters)."""
+        return self.sim.set_origin(*args, **kw)
+
     def stats(self):
         """net.checker stats summed over the shards (every shard counts its own endpoints' events)."""
         import torch

@@ -377,6 +377,7 @@ struct or_sim {
   uint64_t round = 0;
   uint64_t next_id = 0;        // next-message-id starts at -1, first id 0 (net.clj:103,197)
   uint64_t next_event = 0;     // journal next-id (journal.clj:195,228)
+  uint64_t id_origin = 0;      // or_set_origin: the first message id (ids below it were never handed out)
   uint32_t scale = 1;          // slow!/fast! (net.clj:115-119)
   uint64_t loss_thresh = 0;
   std::set<std::pair<uint32_t, uint32_t>> partitions;  // (dest, src), net.clj:109-110
@@ -1354,6 +1355,18 @@ int or_recv(or_sim* s, uint32_t e, int64_t timeout_ns, or_msg* out) {   // net.c
   }
 }
 
+int or_set_origin(or_sim* s, uint64_t round, uint64_t msg_id, uint64_t event_id) {
+  // a fresh simulation only: nothing has been sent, scheduled or run
+  if (s->round || s->next_id != s->id_origin || !s->journal.empty() || !s->host_queue.empty() || !s->schedule.empty()) {
+    s->error = "or_set_origin: the simulation is not fresh";
+    return -2;
+  }
+  s->round = round;
+  s->next_id = s->id_origin = msg_id;
+  s->next_event = event_id;
+  return 0;
+}
+
 int64_t or_now(or_sim* s) { return s->now; }
 uint64_t or_round(or_sim* s) { return s->round; }
 
@@ -1391,14 +1404,15 @@ size_t or_journal_copy(or_sim* s, size_t first, or_event* ev, or_body* bodies, s
 void or_stats(or_sim* s, uint64_t out[9]) {
   // {all,clients,servers} x {send-count, recv-count, msg-count}; msg-count =
   // cardinality of message ids over all events of the class (net/checker.clj:34-36)
-  std::vector<uint8_t> seen(s->next_id, 0);
+  std::vector<uint8_t> seen(s->next_id - s->id_origin, 0);
   uint64_t mc[3] = {0, 0, 0};
   for (const or_event& ev : s->journal) {
     or_msg m; m.src = ev.src; m.dest = ev.dest;
     const bool cl = s->involves_client(m);
     const uint8_t bit = cl ? 2 : 4;
-    if (!(seen[ev.msg_id] & 1)) { seen[ev.msg_id] |= 1; mc[0]++; }
-    if (!(seen[ev.msg_id] & bit)) { seen[ev.msg_id] |= bit; mc[cl ? 1 : 2]++; }
+    uint8_t& sn = seen[ev.msg_id - s->id_origin];
+    if (!(sn & 1)) { sn |= 1; mc[0]++; }
+    if (!(sn & bit)) { sn |= bit; mc[cl ? 1 : 2]++; }
   }
   for (int c = 0; c < 3; c++) {
     out[c * 3 + 0] = s->stats[c * 3 + 0];

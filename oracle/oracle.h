@@ -139,6 +139,10 @@ int      or_run(or_sim*, int64_t until_ns);
 int      or_recv(or_sim*, uint32_t endpoint, int64_t timeout_ns, or_msg* out);
 int64_t  or_now(or_sim*);
 uint64_t or_round(or_sim*);
+/* Start a fresh simulation at round `round`, message id `msg_id` and journal event id `event_id` (the engine's
+ * ms_set_origin without its ring counters, which the oracle does not have).  Journal positions
+ * (or_journal_copy's `first`) stay 0-based. */
+int      or_set_origin(or_sim*, uint64_t round, uint64_t msg_id, uint64_t event_id);
 
 int      or_net_drop(or_sim*, uint32_t src, uint32_t dest);
 int      or_net_heal(or_sim*);

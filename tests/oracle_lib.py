@@ -92,6 +92,7 @@ def lib():
         L.or_now.argtypes = [C.c_void_p]
         L.or_round.restype = C.c_uint64
         L.or_round.argtypes = [C.c_void_p]
+        L.or_set_origin.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64]
         L.or_net_drop.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
         for f in ("or_net_heal", "or_net_slow", "or_net_fast", "or_net_flaky"):
             getattr(L, f).argtypes = [C.c_void_p]
@@ -230,6 +231,10 @@ class Sim:
     @property
     def round(self):
         return self.L.or_round(self.h)
+
+    def set_origin(self, round=0, msg_id=0, event_id=0, ring_pos=0, ring_stride=0):
+        """or_set_origin; ring_pos / ring_stride are the engine's and have no oracle counterpart."""
+        return self._chk(self.L.or_set_origin(self.h, round, msg_id, event_id))
 
     def drop(self, src, dest):
         return self.L.or_net_drop(self.h, src, dest)

@@ -178,10 +178,10 @@ def test_compact_ring_overflow_names_the_receiver():
 
 
 # ------------------------------------------------------------------------------------------- wrap
-@pytest.mark.parametrize("cap", [16, 32])
-def test_windows_wrap_on_both_rings(cap):
-    # small server rings, many rounds: every compact ring wraps several times, and frozen windows straddle the
-    # wrap of the 48-B ring and of the compact ring of the same server in the same round
+def both_rings_wrap(cap):
+    """5-node line with server rings of `cap` records, values to servers 1 and 3 every round for 40 * cap / 16
+    rounds: every compact ring wraps several times.  Returns (engine, oracle, scenario, probes); probes collects
+    the engine's ring counters after each of those rounds."""
     n, rounds = 5, 40 * cap // 16
     g, o = make_pair(n, topology="line", n_values=4096, ring_cap=1024, max_window=256, server_ring_cap=cap,
                      journal_cap_log2=20)
@@ -204,6 +204,15 @@ def test_windows_wrap_on_both_rings(cap):
                 probes.append(s.ring_counters())
         s.run(5_000_000)
 
+    return g, o, scenario, probes
+
+
+@pytest.mark.parametrize("cap", [16, 32])
+def test_windows_wrap_on_both_rings(cap):
+    # small server rings, many rounds: every compact ring wraps several times, and frozen windows straddle the
+    # wrap of the 48-B ring and of the compact ring of the same server in the same round
+    n = 5
+    g, o, scenario, probes = both_rings_wrap(cap)
     both(g, o, scenario)
 
     def straddles(head, limit):

@@ -1,7 +1,8 @@
 """Randomised differential test: seeded random scenarios (topology, latency law, loss, fault
 injections between runs, host sends, scheduled client traffic, sizing near the limits) executed on
 the oracle and on the engine's kernel sources under the CPU SIMT emulator; journals must be
-identical.  `MS_FUZZ_SEEDS=a:b` widens the seed range (the committed default is a handful)."""
+identical.  `MS_FUZZ_SEEDS=a:b` widens the seed range (the committed default is a handful); `MS_FUZZ_ORIGIN=1`
+starts every random, heavy and sharded scenario at a counter origin near a 32-bit boundary (fuzz_origin)."""
 import os
 
 import numpy as np
@@ -34,17 +35,51 @@ def compact_expectation(workload, topology, latency_mean_ms, p_loss, loss_phase=
     return "eq"
 
 
-def assert_gossip_accounting(rings, o, expect):
-    """rings: Sim.ring_counters() of every shard; o: the oracle after the same scenario."""
+def assert_gossip_accounting(rings, o, expect, rings0=None):
+    """rings: Sim.ring_counters() of every shard; o: the oracle after the same scenario; rings0: the counters
+    before it (a ring origin), else they started at 0."""
     ev, bd = o.journal()
     want = oracle_gossip_sends(ev, bd, o.n_nodes)
-    got = sum(compact_total(rc) for rc in rings)
+    if rings0 is None:
+        got = sum(compact_total(rc) for rc in rings)
+    else:                                                     # claims since the start, modulo 2^32
+        got = sum(int((rc["ctail"] - r0["ctail"]).astype(np.uint64).sum()) for rc, r0 in zip(rings, rings0))
     if expect == "eq":
         assert got == want, (got, want)
     elif expect == "le":
         assert got <= want, (got, want)
     else:
         assert got == 0, got
+
+
+def fuzz_origin(seed):
+    """MS_FUZZ_ORIGIN=1: a counter origin (Sim.set_origin) drawn per seed -- message id just below 2^31 or 2^32,
+    event id just below 2^32, round just below 2^15, 2^31 or 2^32, ring counters just below 2^32 with a stride,
+    or all of them -- so that the scenario crosses the boundary; None otherwise."""
+    if os.environ.get("MS_FUZZ_ORIGIN") != "1":
+        return None
+    r = np.random.default_rng(31000 + seed)
+    pick = int(r.integers(6))
+    o = {}
+    if pick in (0, 5):
+        o["msg_id"] = (1 << int(r.choice([31, 32]))) - int(r.integers(1, 3000))
+    if pick in (1, 5):
+        o["event_id"] = (1 << 32) - int(r.integers(1, 6000))
+    if pick in (2, 5):
+        o["round"] = (1 << int(r.choice([15, 31, 32]))) - int(r.integers(1, 60))
+    if pick in (3, 4, 5):
+        o["ring_pos"] = (1 << 32) - int(r.integers(1, 400))
+        o["ring_stride"] = int(r.integers(0, 9))
+    return o
+
+
+def apply_origin(origin, *sims):
+    """Sets `origin` on every sim; returns the engines' ring counters right after (None without an origin)."""
+    if not origin:
+        return None
+    for s in sims:
+        s.set_origin(**origin)
+    return [s.ring_counters() for s in sims if hasattr(s, "ring_counters")]
 
 
 def seeds():
@@ -178,10 +213,12 @@ def test_random_scenario(seed):
 
     with backend():
         g, o = make_pair(n, workload=workload, **kw, **sizing)
+        rings0 = apply_origin(fuzz_origin(seed), g, o)
         rg, ro = both(g, o, scenario)
         assert rg == ro
         loss_phase = any(fault == 5 and int(fault_args[ph][0]) % 40 for ph, (fault, _, _) in enumerate(plan))
-        assert_gossip_accounting([g.ring_counters()], o, compact_expectation(workload, topo, mean, kw["p_loss"], loss_phase))
+        assert_gossip_accounting([g.ring_counters()], o, compact_expectation(workload, topo, mean, kw["p_loss"], loss_phase),
+                                 rings0)
         assert_same_journal(g, o)
 
 
@@ -233,13 +270,14 @@ def test_random_heavy_broadcast(seed):
     with backend():
         import maelstrom_b200 as mb
         g, o = make_pair(n, workload="broadcast", **kw, **sizing)
+        rings0 = apply_origin(fuzz_origin(5000 + seed), g, o)
         try:
             both(g, o, scenario)
         except mb.SimError as e:                              # the random load does not fit this sizing
             if "max_window" in str(e) or "ring overflow" in str(e) or "timing wheel" in str(e):
                 pytest.skip("capacity: %s" % e)
             raise
-        assert_gossip_accounting([g.ring_counters()], o, compact_expectation("broadcast", topo, mean, kw["p_loss"]))
+        assert_gossip_accounting([g.ring_counters()], o, compact_expectation("broadcast", topo, mean, kw["p_loss"]), rings0)
         if sizing["journal_level"] == 2:
             assert_same_journal(g, o)
         else:
@@ -276,9 +314,14 @@ def test_random_sharded(seed):
         kw["gset_interval_ms"] = int(rng.integers(4, 12))
     n_clients = int(rng.integers(1, 5))
     ticks, per_tick = int(rng.integers(3, 10)), int(rng.integers(5, 60))
-    rings = {}
+    rings, rings0 = {}, {}
+    origin = fuzz_origin(9000 + seed)
 
     def scenario(s, body):
+        if origin:
+            s.set_origin(**origin)
+            if hasattr(s, "ring_counters"):
+                rings0[s.cfg.shard_id] = s.ring_counters()
         services = {}
         if workload == "txn-list-append" or rng_services:
             for name in ("lin-kv", "seq-kv", "lin-tso"):
@@ -301,7 +344,8 @@ def test_random_sharded(seed):
     o = O.Sim(n, workload=wl, **kw)
     check_against_oracle(o, scenario, ev, st, now, rnd)
     assert len(rings) == world
-    assert_gossip_accounting(list(rings.values()), o, compact_expectation(workload, kw["topology"], mean, kw["p_loss"]))
+    assert_gossip_accounting([rings[r] for r in range(world)], o, compact_expectation(workload, kw["topology"], mean, kw["p_loss"]),
+                             [rings0[r] for r in range(world)] if origin else None)
 
 
 def raft_seeds():
