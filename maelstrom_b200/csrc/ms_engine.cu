@@ -37,6 +37,7 @@ void msk_journal_expand(const msd::Params* p, uint64_t r0, uint32_t n_rounds, ui
 size_t msk_stream_plan_bytes();
 void msk_stream_batch(const msd::Params* p, void* plan, uint64_t cap_events, uint32_t cap_rounds, ms_jround* rows,
                       void* out, ms_jbatch* hdr, int format, int n_sms, cudaStream_t s, uint32_t parity);
+void msk_stream_mark(const msd::Params* p, void* plan, cudaStream_t s, uint32_t parity);
 void msk_stream_apply(const msd::Params* p, const void* plan, cudaStream_t s, uint32_t parity);
 }
 
@@ -1602,10 +1603,10 @@ int ms_run_streamed(ms_sim* s, int64_t until, int format, size_t buf_events, ms_
   if ((rc = s->set_stop(until))) return rc;
   // the shadow counters start from what has been drained so far
   {
-    struct { uint64_t first, count, r0, n_rounds, jd, dr, jr; uint32_t ov, more; uint64_t local_n, hist[2][3], pad; } init =
+    struct { uint64_t first, count, r0, n_rounds, jd, dr, jr; uint32_t ov, more; uint64_t local_n, hist[2][3], pad, mark[2][4]; } init =
         {0, 0, 0, 0, s->hs.journal_drained, s->hs.drain_round, s->hs.jraw_drained, 0, 0, 0,
-         {{s->hs.journal_drained, s->hs.drain_round, s->hs.jraw_drained}, {s->hs.journal_drained, s->hs.drain_round, s->hs.jraw_drained}}, 0};
-    static_assert(sizeof(init) == 128, "StreamPlan layout");
+         {{s->hs.journal_drained, s->hs.drain_round, s->hs.jraw_drained}, {s->hs.journal_drained, s->hs.drain_round, s->hs.jraw_drained}}, 0, {}};
+    static_assert(sizeof(init) == 128 + 2 * 32, "StreamPlan layout");   // the marks are written before they are read
     CK(cudaMemcpyAsync(s->jplan, &init, sizeof init, cudaMemcpyHostToDevice, s->stream));
     CK(cudaStreamSynchronize(s->stream));
   }
@@ -1629,6 +1630,8 @@ int ms_run_streamed(ms_sim* s, int64_t until, int format, size_t buf_events, ms_
   for (uint64_t i = 0;; i++) {
     const int b = (int)(i & 1), hb = (int)(i & 3);
     if (launching) s->launch_rounds(batch_rounds);
+    // what batch i may pack is fixed here, in stream order: the journal stream runs alongside batch i+1's rounds
+    msk_stream_mark(&s->P, s->jplan, s->stream, (uint32_t)b);
     CK(cudaEventRecord(s->j_rounds_done[b], s->stream));
     CK(cudaStreamWaitEvent(s->jstream, s->j_rounds_done[b], 0));
     msk_stream_batch(&s->P, s->jplan, s->jhost_events, ms_sim::kStreamRows, (ms_jround*)(s->jdev[b] + 256),

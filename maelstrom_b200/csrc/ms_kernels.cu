@@ -2410,6 +2410,17 @@ __global__ void k_journal_expand(Params p, uint64_t r0, uint32_t n_rounds, uint6
 // What has been packed so far lives in StreamPlan (a shadow of DevState's drain counters): the
 // round kernels only ever see the counters k_stream_apply copies over between two rounds, so every
 // kernel of a round takes the same back-pressure decision (round_skipped).
+//
+// The journal stream packs batch i while the rounds of batch i+1 run and commit on the engine stream.
+// So it never reads DevState's live counters: k_stream_mark, on the engine stream right after batch i's
+// rounds, copies them into mark[i & 1], and the journal stream uses that mark plus the rows of rounds
+// below it, which stay as they are until drained.  (Read live, next_event could be ahead of round --
+// commit_scalars stores them in that order -- and jraw_cursor already includes what a running,
+// uncommitted round has claimed: handing that over as drained lets later rounds overwrite it.)
+struct StreamMark {
+  uint64_t round, next_event, raw_base;   // raw_base: jraw_cursor as of the start of round `round`
+  uint32_t error, pad;
+};
 struct StreamPlan {
   uint64_t first, count, r0, n_rounds;
   uint64_t journal_drained, drain_round, jraw_drained;
@@ -2417,29 +2428,46 @@ struct StreamPlan {
   unsigned long long local_n;   // sharded runs: events of this shard appended to the batch so far
   uint64_t hist[2][3];          // the drain counters as of batch i, slot i & 1: what k_stream_apply(i) hands over
   uint64_t pad;
+  StreamMark mark[2];           // the simulation as of the end of batch i's rounds, slot i & 1
 };
-static_assert(sizeof(StreamPlan) == 128, "StreamPlan is initialised from the host");
+static_assert(sizeof(StreamPlan) == 128 + 2 * 32, "StreamPlan is initialised from the host");
 
-__global__ void k_stream_plan(Params p, StreamPlan* plan, uint64_t cap_events, uint32_t cap_rounds, ms_jround* rows, uint32_t format) {
+__global__ void k_stream_mark(Params p, StreamPlan* plan, uint32_t parity) {
   if (threadIdx.x || blockIdx.x) return;
   const DevState* st = p.st;
+  StreamMark mk;
+  mk.round = st->round;
+  mk.next_event = st->next_event;
+  mk.raw_base = p.rmeta[(uint32_t)mk.round & p.hist_mask].raw_base;
+  mk.error = st->error;
+  mk.pad = 0;
+  plan->mark[parity] = mk;
+}
+
+__global__ void k_stream_plan(Params p, StreamPlan* plan, uint64_t cap_events, uint32_t cap_rounds, ms_jround* rows,
+                              uint32_t format, uint32_t parity) {
+  if (threadIdx.x || blockIdx.x) return;
+  const StreamMark mk = plan->mark[parity];
   const uint64_t first = plan->journal_drained;
-  uint64_t count = st->next_event - first;
+  uint64_t count = mk.next_event > first ? mk.next_event - first : 0;
   if (count > cap_events) count = cap_events;
   const uint64_t r0 = plan->drain_round;
-  uint64_t r1 = r0;
-  while (r1 < st->round) {
+  uint64_t r1 = r0, covered = first;      // covered: the end of the events of the rows emitted so far
+  while (r1 < mk.round) {
     const RoundMeta* m = p.rmeta + ((uint32_t)r1 & p.hist_mask);
     if (m->round != r1 || m->ev_base >= first + count) break;
-    if (r1 - r0 >= cap_rounds) { count = m->ev_base - first; break; }   // the rows table is full: cut at the round boundary
+    if (r1 - r0 >= cap_rounds) break;     // the rows table is full: cut at the round boundary
     ms_jround row;
     row.round = r1; row.time_ns = m->now; row.ev_base = m->ev_base;
     // MS_JFMT_4 (one GPU): the round's first message id -- its sends count up from it, its receives down from it
     row.id_ref = (format == MS_JFMT_4 && p.n_shards <= 1) ? m->id_base
                                                           : (m->id_base > (1ull << 30) ? m->id_base - (1ull << 30) : 0ull);
     rows[r1 - r0] = row;
+    covered = m->ev_base + m->ev_total;
     r1++;
   }
+  // an event no row covers would be handed over as whatever the staging buffer held
+  if (count > (covered > first ? covered - first : 0)) count = covered > first ? covered - first : 0;
   plan->first = first; plan->count = count; plan->r0 = r0; plan->n_rounds = r1 - r0;
   plan->overflow = 0;
   plan->local_n = 0;
@@ -2543,26 +2571,29 @@ __global__ void k_journal_pack(Params p, StreamPlan* plan, unsigned char* out) {
 
 __global__ void k_stream_finish(Params p, StreamPlan* plan, ms_jbatch* hdr, uint32_t format, uint32_t parity) {
   if (threadIdx.x || blockIdx.x) return;
+  const StreamMark mk = plan->mark[parity];
   const DevState* st = p.st;
   plan->journal_drained = plan->first + plan->count;
   uint64_t dr = plan->drain_round;
-  while (dr < st->round) {
+  while (dr < mk.round) {
     const RoundMeta* m = p.rmeta + ((uint32_t)dr & p.hist_mask);
     if (m->round != dr || m->ev_base + m->ev_total > plan->journal_drained) break;
     dr++;
   }
   plan->drain_round = dr;
-  plan->jraw_drained = dr < st->round ? p.rmeta[(uint32_t)dr & p.hist_mask].raw_base
-                                      : *reinterpret_cast<const volatile uint64_t*>(&st->jraw_cursor);
-  plan->more = st->next_event > plan->journal_drained ? 1u : 0u;
+  // never past the start of the first round not drained: the rounds running now may have claimed more
+  plan->jraw_drained = dr < mk.round ? p.rmeta[(uint32_t)dr & p.hist_mask].raw_base : mk.raw_base;
+  plan->more = mk.next_event > plan->journal_drained ? 1u : 0u;
   plan->hist[parity][0] = plan->journal_drained;
   plan->hist[parity][1] = plan->drain_round;
   plan->hist[parity][2] = plan->jraw_drained;
   ms_jbatch b;
   b.first_event = plan->first; b.n_events = p.n_shards > 1 ? (uint64_t)plan->local_n : plan->count; b.n_rounds = plan->n_rounds;
-  b.now = st->now; b.round = st->round; b.next_event = st->next_event;
+  // now / round / error only steer the host loop (stop launching, progress, stop on error): the latest values
+  // seen let it stop a batch earlier than the mark would; nothing packed depends on them
+  b.now = st->now; b.round = st->round; b.next_event = mk.next_event;
   b.format = (p.n_shards > 1 && format != MS_JFMT_EVENT) ? (uint32_t)MS_JFMT_16 : format;
-  b.overflow = plan->overflow; b.more = plan->more; b.error = st->error;
+  b.overflow = plan->overflow; b.more = plan->more; b.error = st->error | mk.error;
   b.range_events = plan->count;
   *hdr = b;
   __threadfence_system();
@@ -2689,13 +2720,17 @@ size_t msk_stream_plan_bytes() { return sizeof(msd::StreamPlan); }
 void msk_stream_batch(const msd::Params* p, void* plan, uint64_t cap_events, uint32_t cap_rounds, ms_jround* rows,
                       void* out, ms_jbatch* hdr, int format, int n_sms, cudaStream_t s, uint32_t parity) {
   msd::StreamPlan* pl = (msd::StreamPlan*)plan;
-  MS_LAUNCH(msd::k_stream_plan, 1, 32, 0, s, *p, pl, cap_events, cap_rounds, rows, (uint32_t)format);
+  MS_LAUNCH(msd::k_stream_plan, 1, 32, 0, s, *p, pl, cap_events, cap_rounds, rows, (uint32_t)format, parity);
   const unsigned blocks = (unsigned)n_sms * 16;
   if (format == MS_JFMT_4) MS_LAUNCH(msd::k_journal_pack<4>, blocks, 256, 0, s, *p, pl, (unsigned char*)out);
   else if (format == MS_JFMT_8) MS_LAUNCH(msd::k_journal_pack<8>, blocks, 256, 0, s, *p, pl, (unsigned char*)out);
   else if (format == MS_JFMT_12) MS_LAUNCH(msd::k_journal_pack<12>, blocks, 256, 0, s, *p, pl, (unsigned char*)out);
   else MS_LAUNCH(msd::k_journal_pack<32>, blocks, 256, 0, s, *p, pl, (unsigned char*)out);
   MS_LAUNCH(msd::k_stream_finish, 1, 32, 0, s, *p, pl, hdr, (uint32_t)format, parity);
+}
+// on the engine's stream, behind the rounds of batch `parity`'s parity: what its packing may read
+void msk_stream_mark(const msd::Params* p, void* plan, cudaStream_t s, uint32_t parity) {
+  MS_LAUNCH(msd::k_stream_mark, 1, 32, 0, s, *p, (msd::StreamPlan*)plan, parity);
 }
 void msk_stream_apply(const msd::Params* p, const void* plan, cudaStream_t s, uint32_t parity) {
   MS_LAUNCH(msd::k_stream_apply, 1, 32, 0, s, *p, (const msd::StreamPlan*)plan, parity);

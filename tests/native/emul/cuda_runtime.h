@@ -10,8 +10,17 @@
 // started); the threads of a CTA are fibers switched cooperatively at __syncthreads() and at
 // warp collectives (__shfl*_sync, __match_any_sync, __any_sync), which are evaluated when the
 // last live lane arrives.  Lanes that reach different collectives abort the run (divergence
-// check).  "Device" memory is host memory filled with 0xCD at allocation; streams are
-// synchronous; IPC handles carry the raw pointer, so shards of one process can map each other.
+// check).  "Device" memory is host memory filled with 0xCD at allocation; IPC handles carry the
+// raw pointer, so shards of one process can map each other.
+//
+// Streams are synchronous by default: every launch, copy and memset runs when it is enqueued.
+// MS_EMUL_STREAMS=<seed> (or simt_streams(seed) at run time) makes them asynchronous: each stream
+// is a FIFO of launches, async copies, memsets and event records; cudaStreamWaitEvent is a
+// dependency on the recorded position; host synchronisation runs the queues up to the point it
+// waits for (synchronous copies drain everything).  A seeded choice may start another stream's
+// ready work first, and at a __syncthreads() of a running kernel may run another stream's ready
+// work to completion while the CTA is parked (one nesting level).  So the journal stream of
+// ms_run_streamed can read the state while a round of the next batch is half done.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -120,14 +129,26 @@ static inline unsigned max(unsigned a, unsigned b) { return a > b ? a : b; }
 static inline unsigned long max(unsigned long a, unsigned long b) { return a > b ? a : b; }
 static inline long max(long a, long b) { return a > b ? a : b; }
 
-// kernel launch: MS_LAUNCH(kernel, grid, block, dynamic smem bytes, stream, args...)
-#define MS_LAUNCH(kern, grid, block, smem, stream, ...) \
-  simt::launch((unsigned)(grid), (unsigned)(block), (size_t)(smem), [&]() { kern(__VA_ARGS__); })
+typedef struct simt_stream* cudaStream_t;
+
+namespace simt {
+// the arguments are evaluated and copied when the launch is enqueued, as a CUDA launch does
+template <class K, class... A> static inline std::function<void()> bind_kernel(K k, A... a) {
+  return [=]() { k(a...); };
+}
+void enqueue_launch(cudaStream_t s, const void* kern, unsigned grid, unsigned block, size_t dyn_smem,
+                    std::function<void()> body);
+}  // namespace simt
+
+// kernel launch: MS_LAUNCH(kernel, grid, block, dynamic smem bytes, stream, args...).  Runs at once, or
+// under MS_EMUL_STREAMS queues on its stream (simt.cpp).
+#define MS_LAUNCH(kern, grid, block, smem, stream, ...)                                                 \
+  simt::enqueue_launch((stream), (const void*)(kern), (unsigned)(grid), (unsigned)(block), (size_t)(smem), \
+                       simt::bind_kernel(kern, __VA_ARGS__))
 
 // ---------------------------------------------------------------- runtime API subset
 typedef int cudaError_t;
 enum { cudaSuccess = 0, cudaErrorInvalidValue = 1, cudaErrorMemoryAllocation = 2, cudaErrorNotSupported = 801 };
-typedef struct simt_stream* cudaStream_t;
 typedef struct simt_event* cudaEvent_t;
 typedef struct simt_graph* cudaGraph_t;
 typedef struct simt_graph_exec* cudaGraphExec_t;

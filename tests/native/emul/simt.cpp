@@ -4,7 +4,15 @@
 #include <stdio.h>
 #include <sys/mman.h>
 
+#include <dlfcn.h>
+
+#include <algorithm>
+#include <atomic>
 #include <chrono>
+#include <deque>
+#include <map>
+#include <memory>
+#include <mutex>
 #include <thread>
 #include <vector>
 
@@ -89,18 +97,25 @@ struct Sched {
   char sync_warp[kMaxThreads / 32];
   unsigned bar_calls[kMaxThreads];   // MS_TSAN self-test
 };
-static thread_local Sched* g_s = nullptr;
+static thread_local Sched* g_s = nullptr;          // the scheduler of the launch that runs now
+static thread_local Sched* g_top = nullptr;        // top-level launches
+static thread_local Sched* g_nested = nullptr;     // MS_EMUL_STREAMS: work run while a top-level CTA is parked
+
+static Sched* new_sched() {
+  Sched* s = new Sched();
+  s->stacks = (char*)mmap(nullptr, (size_t)kMaxThreads * kStack, PROT_READ | PROT_WRITE,
+                          MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
+  if (s->stacks == (char*)MAP_FAILED) { fprintf(stderr, "simt: mmap failed\n"); abort(); }
+  if (posix_memalign((void**)&s->smem, 128, 256 << 10)) abort();
+  return s;
+}
 
 static Sched* sched() {
-  if (!g_s) {
-    g_s = new Sched();
-    g_s->stacks = (char*)mmap(nullptr, (size_t)kMaxThreads * kStack, PROT_READ | PROT_WRITE,
-                              MAP_PRIVATE | MAP_ANONYMOUS | MAP_NORESERVE, -1, 0);
-    if (g_s->stacks == (char*)MAP_FAILED) { fprintf(stderr, "simt: mmap failed\n"); abort(); }
-    if (posix_memalign((void**)&g_s->smem, 128, 256 << 10)) abort();
-  }
+  if (!g_s) g_s = g_top = new_sched();
   return g_s;
 }
+
+static void maybe_interleave();   // MS_EMUL_STREAMS, below
 
 [[noreturn]] static void die(const char* what) {
   fprintf(stderr, "simt emulator: %s (block %u thread %u)\n", what, tls.bid.x, tls.tid.x);
@@ -149,6 +164,7 @@ void sync_threads() { (void)barrier(0, true); }
 int sync_threads_or(int pred) { return barrier(pred, false); }
 
 static int barrier(int pred, bool plain) {
+  maybe_interleave();
   Sched* s = g_s;
 #ifdef MS_TSAN
   // self-test of the race check: MS_TSAN_SKIP_BARRIER=k turns every k-th barrier of every CTA into
@@ -336,14 +352,220 @@ static void launch_impl(unsigned grid, unsigned block, size_t dyn, const std::fu
 
 }  // namespace simt
 
+// ------------------------------------------------------------------ MS_EMUL_STREAMS: asynchronous streams
+// A stream is a FIFO of operations owned by the host thread that enqueued them; event k of a stream is
+// complete once `done` has reached its position.  Nothing runs out of stream order, nothing runs before a
+// cudaStreamWaitEvent dependency is met; apart from that the seeded choices below decide what runs when.
+struct simt_stream;
+struct simt_event {
+  std::chrono::steady_clock::time_point t;
+  simt_stream* s = nullptr;   // the stream and position of the last record (nullptr: complete)
+  uint64_t seq = 0;
+};
+struct simt_op {
+  enum Kind { LAUNCH, WORK, RECORD, WAIT } kind;
+  std::function<void()> fn;   // LAUNCH: the kernel body; WORK: a copy or memset
+  const void* kern = nullptr;
+  unsigned grid = 0, block = 0;
+  size_t dyn = 0;
+  simt_event* ev = nullptr;   // RECORD
+  simt_stream* dep = nullptr; // WAIT: (stream, position) of the awaited record, fixed when enqueued
+  uint64_t dep_seq = 0;
+};
+struct simt_stream {
+  std::deque<simt_op> q;
+  uint64_t enq = 0, done = 0;
+  std::thread::id owner;
+};
+
+namespace simt {
+
+static std::mutex g_reg_mu;                        // the stream registry and the interleave counters
+static std::vector<simt_stream*> g_streams;
+static std::map<std::pair<const void*, const void*>, uint64_t> g_pairs;   // (parked kernel, kernel run meanwhile)
+static std::atomic<int64_t> g_seed{-2};            // -2: not read yet, -1: synchronous streams
+static std::atomic<uint64_t> g_seed_gen{0};
+static thread_local uint64_t t_rng = 0, t_rng_gen = ~0ull;
+static thread_local simt_stream* t_run_stream = nullptr;   // stream of the top-level launch running now
+static thread_local const void* t_run_kern = nullptr;
+static thread_local bool t_nested = false;
+
+static bool streams_async() {
+  int64_t v = g_seed.load();
+  if (v == -2) {
+    const char* e = getenv("MS_EMUL_STREAMS");
+    int64_t want = (e && *e) ? (int64_t)strtoull(e, nullptr, 0) : -1;
+    g_seed.compare_exchange_strong(v, want);
+    v = g_seed.load();
+  }
+#ifdef MS_TSAN
+  return false;      // the TSan fiber bookkeeping assumes one launch at a time
+#else
+  return v >= 0;
+#endif
+}
+
+static uint64_t rng() {                            // splitmix64 of the seed, per host thread
+  if (t_rng_gen != g_seed_gen.load()) { t_rng = (uint64_t)g_seed.load(); t_rng_gen = g_seed_gen.load(); }
+  uint64_t z = (t_rng += 0x9E3779B97F4A7C15ull);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+static bool dep_met(const simt_op& op) { return op.dep == nullptr || op.dep->done >= op.dep_seq; }
+
+static void exec_head(simt_stream* st);
+static void run_until(simt_stream* st, uint64_t seq);
+
+static void run_launch(simt_stream* st, const simt_op& op) {
+  simt_stream* const ps = t_run_stream;
+  const void* const pk = t_run_kern;
+  if (!t_nested) { t_run_stream = st; t_run_kern = op.kern; }
+  launch(op.grid, op.block, op.dyn, op.fn);
+  t_run_stream = ps; t_run_kern = pk;
+}
+
+static void exec_head(simt_stream* st) {
+  simt_op op = std::move(st->q.front());
+  st->q.pop_front();
+  switch (op.kind) {
+    case simt_op::LAUNCH: run_launch(st, op); break;
+    case simt_op::WORK: op.fn(); break;
+    case simt_op::RECORD: op.ev->t = std::chrono::steady_clock::now(); break;
+    case simt_op::WAIT:
+      if (!dep_met(op)) {
+        if (t_nested) die("MS_EMUL_STREAMS: nested work waits on an event");
+        run_until(op.dep, op.dep_seq);
+      }
+      break;
+  }
+  st->done++;
+}
+
+// streams of this host thread (other than `except`) whose next operation may run now, skipping launches of
+// `not_kern` (its __shared__ statics are in use by the parked CTA)
+static simt_stream* pick_ready(simt_stream* except, const void* not_kern) {
+  std::vector<simt_stream*> ready;
+  {
+    std::lock_guard<std::mutex> g(g_reg_mu);
+    const std::thread::id me = std::this_thread::get_id();
+    for (simt_stream* st : g_streams) {
+      if (st == except || st->owner != me || st->q.empty()) continue;
+      const simt_op& h = st->q.front();
+      if (h.kind == simt_op::WAIT && !dep_met(h)) continue;
+      if (h.kind == simt_op::LAUNCH && not_kern && h.kern == not_kern) continue;
+      ready.push_back(st);
+    }
+  }
+  return ready.empty() ? nullptr : ready[rng() % ready.size()];
+}
+
+static void run_until(simt_stream* st, uint64_t seq) {
+  while (st->done < seq) {
+    if (st->q.empty()) die("MS_EMUL_STREAMS: waiting for work that was never enqueued");
+    const simt_op& h = st->q.front();
+    if (h.kind == simt_op::WAIT && !dep_met(h)) { run_until(h.dep, h.dep_seq); continue; }
+    if (!t_nested && (rng() & 1)) {            // the GPU may as well have started another stream's work first
+      if (simt_stream* o = pick_ready(st, nullptr)) { exec_head(o); continue; }
+    }
+    exec_head(st);
+  }
+}
+
+static void drain_all() {
+  if (!streams_async()) return;
+  if (t_nested) die("MS_EMUL_STREAMS: host synchronisation inside a kernel");
+  for (;;) {
+    simt_stream* pending = nullptr;
+    {
+      std::lock_guard<std::mutex> g(g_reg_mu);
+      const std::thread::id me = std::this_thread::get_id();
+      for (simt_stream* st : g_streams)
+        if (st->owner == me && !st->q.empty()) { pending = st; break; }
+    }
+    if (!pending) return;
+    run_until(pending, pending->enq);
+  }
+}
+
+static void push(simt_stream* st, simt_op op) {
+  st->owner = std::this_thread::get_id();
+  st->q.push_back(std::move(op));
+  st->enq++;
+}
+
+// at a __syncthreads() of a top-level kernel: maybe run one ready operation of another stream to completion
+static void maybe_interleave() {
+  if (t_nested || !t_run_stream || g_s != g_top || !streams_async()) return;
+  if (rng() % 8) return;
+  simt_stream* o = pick_ready(t_run_stream, t_run_kern);
+  if (!o) return;
+  if (o->q.front().kind == simt_op::LAUNCH) {
+    std::lock_guard<std::mutex> g(g_reg_mu);
+    g_pairs[{t_run_kern, o->q.front().kern}]++;
+  }
+  if (!g_nested) g_nested = new_sched();
+  const Tls saved = tls;
+  g_s = g_nested;
+  t_nested = true;
+  exec_head(o);
+  t_nested = false;
+  g_s = g_top;
+  tls = saved;
+}
+
+void enqueue_launch(cudaStream_t st, const void* kern, unsigned grid, unsigned block, size_t dyn,
+                    std::function<void()> body) {
+  if (!st || !streams_async() || t_nested) {   // nested work launches nothing, so this is host code
+    drain_all();
+    launch(grid, block, dyn, body);
+    return;
+  }
+  simt_op op{simt_op::LAUNCH};
+  op.fn = std::move(body);
+  op.kern = kern; op.grid = grid; op.block = block; op.dyn = dyn;
+  push(st, std::move(op));
+}
+
+}  // namespace simt
+
+// test hooks (tests/test_stream_overlap.py): switch the stream mode at run time, and count the kernels that
+// ran while a top-level CTA was parked, by (parked kernel, kernel) symbol substrings
+extern "C" void simt_streams(long long seed) {
+  simt::drain_all();
+  simt::g_seed.store(seed < 0 ? -1 : seed);
+  simt::g_seed_gen++;
+}
+extern "C" unsigned long long simt_interleaved(const char* parked, const char* ran) {
+  std::lock_guard<std::mutex> g(simt::g_reg_mu);
+  unsigned long long n = 0;
+  for (const auto& kv : simt::g_pairs) {
+    Dl_info a{}, b{};
+    if (!dladdr(kv.first.first, &a) || !dladdr(kv.first.second, &b) || !a.dli_sname || !b.dli_sname) continue;
+    if (strstr(a.dli_sname, parked) && strstr(b.dli_sname, ran)) n += kv.second;
+  }
+  return n;
+}
+extern "C" void simt_interleaved_reset() {
+  std::lock_guard<std::mutex> g(simt::g_reg_mu);
+  simt::g_pairs.clear();
+}
+
 long long clock64() {
   return (long long)std::chrono::duration_cast<std::chrono::nanoseconds>(
              std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
 // -------------------------------------------------------------------- runtime API stubs
-struct simt_event { std::chrono::steady_clock::time_point t; };
-struct simt_stream { int unused; };
+using simt::drain_all;
+using simt::streams_async;
+
+static simt_op work_op(std::function<void()> fn) {
+  simt_op op{simt_op::WORK};
+  op.fn = std::move(fn);
+  return op;
+}
 
 const char* cudaGetErrorString(cudaError_t e) {
   switch (e) {
@@ -373,15 +595,51 @@ cudaError_t cudaMalloc(void** p, size_t bytes) {
   *p = q;
   return cudaSuccess;
 }
-cudaError_t cudaFree(void* p) { free(p); return cudaSuccess; }
-cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { memmove(d, s, n); return cudaSuccess; }
-cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t) { memmove(d, s, n); return cudaSuccess; }
-cudaError_t cudaMemset(void* d, int v, size_t n) { memset(d, v, n); return cudaSuccess; }
-cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t) { memset(d, v, n); return cudaSuccess; }
-cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = new simt_stream(); return cudaSuccess; }
-cudaError_t cudaStreamDestroy(cudaStream_t s) { delete s; return cudaSuccess; }
-cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
-cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, unsigned) { return cudaSuccess; }
+cudaError_t cudaFree(void* p) { drain_all(); free(p); return cudaSuccess; }
+cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { drain_all(); memmove(d, s, n); return cudaSuccess; }
+cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind k, cudaStream_t st) {
+  if (!st || !streams_async()) { drain_all(); memmove(d, s, n); return cudaSuccess; }
+  if (k == cudaMemcpyHostToDevice) {          // the source is taken when the copy is enqueued (it may be on the stack)
+    auto src = std::make_shared<std::vector<unsigned char>>((const unsigned char*)s, (const unsigned char*)s + n);
+    simt::push(st, work_op([=]() { memmove(d, src->data(), n); }));
+  } else {
+    simt::push(st, work_op([=]() { memmove(d, s, n); }));
+  }
+  return cudaSuccess;
+}
+cudaError_t cudaMemset(void* d, int v, size_t n) { drain_all(); memset(d, v, n); return cudaSuccess; }
+cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t st) {
+  if (!st || !streams_async()) { drain_all(); memset(d, v, n); return cudaSuccess; }
+  simt::push(st, work_op([=]() { memset(d, v, n); }));
+  return cudaSuccess;
+}
+cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) {
+  *s = new simt_stream();
+  std::lock_guard<std::mutex> g(simt::g_reg_mu);
+  simt::g_streams.push_back(*s);
+  return cudaSuccess;
+}
+cudaError_t cudaStreamDestroy(cudaStream_t s) {
+  if (streams_async()) simt::run_until(s, s->enq);
+  std::lock_guard<std::mutex> g(simt::g_reg_mu);
+  simt::g_streams.erase(std::find(simt::g_streams.begin(), simt::g_streams.end(), s));
+  // the object stays: an event may still name it (as complete: done == enq)
+  return cudaSuccess;
+}
+cudaError_t cudaStreamSynchronize(cudaStream_t s) {
+  if (!streams_async()) return cudaSuccess;
+  if (!s) drain_all();
+  else simt::run_until(s, s->enq);
+  return cudaSuccess;
+}
+cudaError_t cudaStreamWaitEvent(cudaStream_t s, cudaEvent_t e, unsigned) {
+  if (!streams_async() || !e->s) return cudaSuccess;
+  if (!s) { simt::run_until(e->s, e->seq); return cudaSuccess; }
+  simt_op op{simt_op::WAIT};
+  op.dep = e->s; op.dep_seq = e->seq;
+  simt::push(s, std::move(op));
+  return cudaSuccess;
+}
 cudaError_t cudaStreamIsCapturing(cudaStream_t, cudaStreamCaptureStatus* st) { *st = cudaStreamCaptureStatusNone; return cudaSuccess; }
 cudaError_t cudaStreamBeginCapture(cudaStream_t, cudaStreamCaptureMode) { return cudaErrorNotSupported; }
 cudaError_t cudaStreamEndCapture(cudaStream_t, cudaGraph_t* g) { *g = nullptr; return cudaErrorNotSupported; }
@@ -391,9 +649,25 @@ cudaError_t cudaGraphDestroy(cudaGraph_t) { return cudaSuccess; }
 cudaError_t cudaGraphExecDestroy(cudaGraphExec_t) { return cudaSuccess; }
 cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = new simt_event(); return cudaSuccess; }
 cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned) { *e = new simt_event(); return cudaSuccess; }
-cudaError_t cudaEventDestroy(cudaEvent_t e) { delete e; return cudaSuccess; }
-cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t) { e->t = std::chrono::steady_clock::now(); return cudaSuccess; }
-cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
+cudaError_t cudaEventDestroy(cudaEvent_t e) { drain_all(); delete e; return cudaSuccess; }
+cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t s) {
+  if (!s || !streams_async()) {
+    drain_all();
+    e->t = std::chrono::steady_clock::now();
+    e->s = nullptr;
+    return cudaSuccess;
+  }
+  simt_op op{simt_op::RECORD};
+  op.ev = e;
+  simt::push(s, std::move(op));
+  e->s = s;
+  e->seq = s->enq;
+  return cudaSuccess;
+}
+cudaError_t cudaEventSynchronize(cudaEvent_t e) {
+  if (streams_async() && e->s) simt::run_until(e->s, e->seq);
+  return cudaSuccess;
+}
 cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t a, cudaEvent_t b) {
   *ms = std::chrono::duration<float, std::milli>(b->t - a->t).count();
   return cudaSuccess;
