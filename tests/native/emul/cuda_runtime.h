@@ -6,8 +6,8 @@
 // directory first on the include path and defines MS_EMUL.  Nothing in maelstrom_b200/ loads
 // the resulting library: the product has no CPU path.
 //
-// Model: CTAs of a launch run one after another (the kernels never wait on a CTA that has not
-// started); the threads of a CTA are fibers switched cooperatively at __syncthreads() and at
+// Model: CTAs of a launch run one after another by default (the kernels never wait on a CTA that has not
+// started; MS_EMUL_CTAS below runs them concurrently); the threads of a CTA are fibers switched cooperatively at __syncthreads() and at
 // warp collectives (__shfl*_sync, __match_any_sync, __any_sync), which are evaluated when the
 // last live lane arrives.  Lanes that reach different collectives abort the run (divergence
 // check).  "Device" memory is host memory filled with 0xCD at allocation; IPC handles carry the
@@ -21,6 +21,16 @@
 // ready work first, and at a __syncthreads() of a running kernel may run another stream's ready
 // work to completion while the CTA is parked (one nesting level).  So the journal stream of
 // ms_run_streamed can read the state while a round of the next batch is half done.
+//
+// MS_EMUL_CTAS=<seed> (or simt_ctas(seed) at run time; -1 = off, the default) runs the CTAs of a launch of two or
+// more concurrently: a pool of host threads per launching thread, 2 x MS_EMUL_SMS CTAs resident at once (one per
+// thread, with its own fibers and, __shared__ being thread_local, its own shared memory), a finished CTA's thread
+// taking the next block index.  A baton lets one thread run at a time, so a run is a function of the seed.  At a
+// CTA's start, its first arrival at a __syncthreads(), every atomic*, __threadfence* and every spin-wait
+// (__nanosleep / relax) a seeded choice may park the whole CTA and resume another; a parked CTA may be held for
+// many switches.  All of them live in this directory: the kernel sources are compiled as they are.  Combined with MS_EMUL_STREAMS, nested stream work runs
+// on the parked CTA's thread.  Stores still land in program order at once: no reordering between SMs.  The TSan
+// build keeps sequential CTAs.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -63,6 +73,13 @@ int sync_threads_or(int pred);
 enum Op { OP_SHFL_UP = 1, OP_SHFL_XOR, OP_SHFL_IDX, OP_MATCH_ANY, OP_ANY, OP_BALLOT };
 uint64_t warp_op(int op, unsigned mask, uint64_t v, int arg);
 void relax();   // spin-wait hint: lets other host threads (shards) run
+// MS_EMUL_CTAS: the places where a CTA of a concurrent launch may be parked for another one (simt.cpp)
+enum Switch { SW_START, SW_BARRIER, SW_ATOMIC, SW_FENCE, SW_SPIN };
+extern thread_local bool in_cta_pool;   // this host thread runs a CTA of a launch with several resident
+void cta_switch(int why);
+static inline void cta_point(int why) {
+  if (in_cta_pool) cta_switch(why);
+}
 }  // namespace simt
 
 #define threadIdx (simt::tls.tid)
@@ -102,19 +119,33 @@ template <class T> static inline T __ldcg(const T* p) {
   return v;
 }
 template <class T, class U> static inline void __stcg(T* p, U v) { *(volatile T*)p = (T)v; }
-static inline void __threadfence() { __atomic_thread_fence(__ATOMIC_SEQ_CST); }
-static inline void __threadfence_system() { __atomic_thread_fence(__ATOMIC_SEQ_CST); }
+static inline void __threadfence() {
+  simt::cta_point(simt::SW_FENCE);
+  __atomic_thread_fence(__ATOMIC_SEQ_CST);
+}
+static inline void __threadfence_system() {
+  simt::cta_point(simt::SW_FENCE);
+  __atomic_thread_fence(__ATOMIC_SEQ_CST);
+}
 static inline void __nanosleep(unsigned) { simt::relax(); }
 long long clock64();
 
-template <class T, class U> static inline T atomicAdd(T* p, U v) { return __atomic_fetch_add(p, (T)v, __ATOMIC_SEQ_CST); }
-template <class T, class U> static inline T atomicOr(T* p, U v) { return __atomic_fetch_or(p, (T)v, __ATOMIC_SEQ_CST); }
+template <class T, class U> static inline T atomicAdd(T* p, U v) {
+  simt::cta_point(simt::SW_ATOMIC);
+  return __atomic_fetch_add(p, (T)v, __ATOMIC_SEQ_CST);
+}
+template <class T, class U> static inline T atomicOr(T* p, U v) {
+  simt::cta_point(simt::SW_ATOMIC);
+  return __atomic_fetch_or(p, (T)v, __ATOMIC_SEQ_CST);
+}
 template <class T, class U> static inline T atomicMax(T* p, U v) {
+  simt::cta_point(simt::SW_ATOMIC);
   T cur = __atomic_load_n(p, __ATOMIC_SEQ_CST);
   while (cur < (T)v && !__atomic_compare_exchange_n(p, &cur, (T)v, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST)) {}
   return cur;
 }
 template <class T, class U, class V> static inline T atomicCAS(T* p, U cmp, V val) {
+  simt::cta_point(simt::SW_ATOMIC);
   T expected = (T)cmp;
   __atomic_compare_exchange_n(p, &expected, (T)val, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST);
   return expected;

@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <condition_variable>
 #include <deque>
 #include <map>
 #include <memory>
@@ -116,6 +117,7 @@ static Sched* sched() {
 }
 
 static void maybe_interleave();   // MS_EMUL_STREAMS, below
+thread_local bool in_cta_pool = false;   // MS_EMUL_CTAS, below
 
 [[noreturn]] static void die(const char* what) {
   fprintf(stderr, "simt emulator: %s (block %u thread %u)\n", what, tls.bid.x, tls.tid.x);
@@ -164,6 +166,7 @@ void sync_threads() { (void)barrier(0, true); }
 int sync_threads_or(int pred) { return barrier(pred, false); }
 
 static int barrier(int pred, bool plain) {
+  if (in_cta_pool && g_s->bar_count == 0) cta_switch(SW_BARRIER);   // the CTA's first thread to arrive
   maybe_interleave();
   Sched* s = g_s;
 #ifdef MS_TSAN
@@ -240,6 +243,7 @@ void relax() {
   // a spin-wait (k_barrier polling a peer's flag): let the other host threads (shards) run AND
   // the other fibers of this CTA, which on a GPU would be running concurrently
   std::this_thread::yield();
+  if (in_cta_pool) cta_switch(SW_SPIN);   // ... and the other resident CTAs of this launch
   if (g_s && g_s->body) {
     g_s->progress++;
     yield_to_scheduler();
@@ -329,11 +333,14 @@ void launch(unsigned grid, unsigned block, size_t dyn, const std::function<void(
   g_prof[i].n++;
   g_prof[i].sec += dt;
 }
+static bool ctas_launch(unsigned grid, unsigned block, size_t dyn, const std::function<void()>& body);
 static void launch_impl(unsigned grid, unsigned block, size_t dyn, const std::function<void()>& body) {
-  Sched* s = sched();
-  if (s->body) die("nested kernel launch");
   if (block == 0 || block > kMaxThreads) die("bad block size");
   if (dyn > (256u << 10)) die("dynamic shared memory too large");
+  if (in_cta_pool) die("nested kernel launch");
+  if (ctas_launch(grid, block, dyn, body)) return;
+  Sched* s = sched();
+  if (s->body) die("nested kernel launch");
   s->body = &body;
   tls.bdim = dim3{block, 1, 1};
   tls.gdim = dim3{grid, 1, 1};
@@ -389,6 +396,8 @@ static thread_local uint64_t t_rng = 0, t_rng_gen = ~0ull;
 static thread_local simt_stream* t_run_stream = nullptr;   // stream of the top-level launch running now
 static thread_local const void* t_run_kern = nullptr;
 static thread_local bool t_nested = false;
+static thread_local const void* t_kern = nullptr;          // the kernel launch() is about to run (MS_EMUL_CTAS counters)
+static std::thread::id host_thread();                      // MS_EMUL_CTAS: the thread that launched, seen from a worker
 
 static bool streams_async() {
   int64_t v = g_seed.load();
@@ -422,6 +431,7 @@ static void run_launch(simt_stream* st, const simt_op& op) {
   simt_stream* const ps = t_run_stream;
   const void* const pk = t_run_kern;
   if (!t_nested) { t_run_stream = st; t_run_kern = op.kern; }
+  t_kern = op.kern;
   launch(op.grid, op.block, op.dyn, op.fn);
   t_run_stream = ps; t_run_kern = pk;
 }
@@ -449,7 +459,7 @@ static simt_stream* pick_ready(simt_stream* except, const void* not_kern) {
   std::vector<simt_stream*> ready;
   {
     std::lock_guard<std::mutex> g(g_reg_mu);
-    const std::thread::id me = std::this_thread::get_id();
+    const std::thread::id me = host_thread();
     for (simt_stream* st : g_streams) {
       if (st == except || st->owner != me || st->q.empty()) continue;
       const simt_op& h = st->q.front();
@@ -507,9 +517,12 @@ static void maybe_interleave() {
   }
   if (!g_nested) g_nested = new_sched();
   const Tls saved = tls;
+  const bool pooled = in_cta_pool;
   g_s = g_nested;
   t_nested = true;
+  in_cta_pool = false;       // MS_EMUL_CTAS: the nested work runs to completion before any other CTA resumes
   exec_head(o);
+  in_cta_pool = pooled;
   t_nested = false;
   g_s = g_top;
   tls = saved;
@@ -519,6 +532,7 @@ void enqueue_launch(cudaStream_t st, const void* kern, unsigned grid, unsigned b
                     std::function<void()> body) {
   if (!st || !streams_async() || t_nested) {   // nested work launches nothing, so this is host code
     drain_all();
+    t_kern = kern;
     launch(grid, block, dyn, body);
     return;
   }
@@ -528,7 +542,211 @@ void enqueue_launch(cudaStream_t st, const void* kern, unsigned grid, unsigned b
   push(st, std::move(op));
 }
 
+// ------------------------------------------------------------------ MS_EMUL_CTAS: CTAs of a launch concurrently
+// A launch of two or more CTAs runs on a pool of worker host threads that belongs to the launching host thread
+// (a shard has its own): one resident CTA per worker, 2 x MS_EMUL_SMS workers (a persistent k_round grid is SMs x
+// one CTA, so it is fully resident), and a worker whose CTA finishes takes the next block index.  Each worker has
+// its own fiber scheduler and, through thread_local, its own __shared__ statics.  A baton lets exactly one thread
+// of the pool (or the launcher) run at a time, so a run is a function of the seed: at each switch point a seeded
+// choice may park the whole running CTA and hand the baton to another resident one.  A spin-wait always offers it.
+struct CtaPool {
+  std::mutex mu;
+  std::condition_variable cv;
+  int turn = -1;                  // who holds the baton: a worker, or -1 = the launching thread
+  bool quit = false;
+  std::vector<std::thread> threads;
+  std::vector<int> block;         // per worker: the block index of its CTA, -1 = none
+  std::vector<int> hold;          // per worker: passes it stays parked for
+  std::thread::id owner;
+  // the launch in progress
+  const std::function<void()>* body = nullptr;
+  unsigned grid = 0, nthreads = 0, next = 0;
+  size_t dyn = 0;
+  simt_stream* run_stream = nullptr;
+  const void* run_kern = nullptr;
+  uint64_t passes = 0;            // baton passes from a CTA that had started and not finished
+  uint64_t rng = 0, rng_gen = ~0ull;
+  ~CtaPool() {
+    { std::lock_guard<std::mutex> g(mu); quit = true; }
+    cv.notify_all();
+    for (auto& t : threads) t.join();
+  }
+};
+static std::atomic<int64_t> g_cta_seed{-2};       // -2: not read yet, -1: off
+static std::atomic<uint64_t> g_cta_gen{0};
+static std::mutex g_cta_mu;                        // the counters below
+static std::map<const void*, std::pair<uint64_t, uint64_t>> g_cta_counts;   // kernel -> (overlapped launches, passes)
+static thread_local std::unique_ptr<CtaPool> t_own_pool;   // on a launching thread
+static thread_local CtaPool* t_pool = nullptr;             // on a worker: its pool
+static thread_local int t_worker = -1;
+
+static std::thread::id host_thread() { return t_pool ? t_pool->owner : std::this_thread::get_id(); }
+
+static bool ctas_on() {
+  int64_t v = g_cta_seed.load();
+  if (v == -2) {
+    const char* e = getenv("MS_EMUL_CTAS");
+    int64_t want = (e && *e) ? (int64_t)strtoll(e, nullptr, 0) : -1;
+    if (want < -1) want = -1;
+    g_cta_seed.compare_exchange_strong(v, want);
+    v = g_cta_seed.load();
+  }
+#ifdef MS_TSAN
+  return false;      // the TSan build keeps CTAs sequential (their __shared__ statics are chained on purpose)
+#else
+  return v >= 0;
+#endif
+}
+
+static uint64_t cta_rng(CtaPool* P) {
+  if (P->rng_gen != g_cta_gen.load()) { P->rng = (uint64_t)g_cta_seed.load() * 0x2545F4914F6CDD1Dull; P->rng_gen = g_cta_gen.load(); }
+  uint64_t z = (P->rng += 0x9E3779B97F4A7C15ull);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// hands the baton to `to` and waits until it comes back (under the pool's lock: the hand-over orders memory)
+static void hand_over(CtaPool* P, int to, int me) {
+  std::unique_lock<std::mutex> lk(P->mu);
+  P->turn = to;
+  P->cv.notify_all();
+  P->cv.wait(lk, [&] { return P->turn == me; });
+}
+
+void cta_switch(int why) {
+  CtaPool* P = t_pool;
+  const int me = t_worker;
+  bool any = false;
+  for (int w = 0; w < (int)P->block.size() && !any; w++) any = w != me && P->block[w] >= 0;
+  if (!any) return;
+  const uint64_t r = cta_rng(P);
+  // how often each switch point passes: a CTA start one time in two, the CTA's first arrival at a barrier one in
+  // four, an atomic or fence one in eight, a spin-wait always
+  static const unsigned mask[] = {1, 3, 7, 7, 0};
+  if (r & mask[why]) return;
+  // A CTA parked here stays parked for the next 512-1535 switches one time in eight, and for 32-95 of them one time
+  // in eight: an SM busy elsewhere, which is what lets a bounded poll such as wheel_block's give up on its publisher.
+  // Held CTAs are passed over; a spin-wait that finds nobody else counts down their holds instead (so an unbounded
+  // wait still reaches them), any other switch point takes a held CTA when nobody else is left.
+  for (int& h : P->hold)
+    if (h > 0) h--;
+  if (why != SW_SPIN) {
+    if (((r >> 40) & 7) == 1) P->hold[me] = 512 + (int)((r >> 45) & 1023);
+    else if (((r >> 40) & 7) == 0) P->hold[me] = 32 + (int)((r >> 45) & 63);
+  }
+  int cand[256], n = 0;
+  for (int pass = 0; pass < (why == SW_SPIN ? 1 : 2) && n == 0; pass++)
+    for (int w = 0; w < (int)P->block.size(); w++)
+      if (w != me && P->block[w] >= 0 && (pass || P->hold[w] == 0)) cand[n++] = w;
+  if (!n) return;
+  if (why != SW_START) P->passes++;
+  hand_over(P, cand[(r >> 16) % (uint64_t)n], me);
+}
+
+static void free_sched(Sched* s) {
+  if (!s) return;
+  munmap(s->stacks, (size_t)kMaxThreads * kStack);
+  free(s->smem);
+  delete s;
+}
+
+static void cta_worker(CtaPool* P, int me) {
+  t_pool = P;
+  t_worker = me;
+  g_s = g_top = new_sched();
+  std::unique_lock<std::mutex> lk(P->mu);
+  for (;;) {
+    P->cv.wait(lk, [&] { return P->turn == me || P->quit; });
+    if (P->quit) break;
+    lk.unlock();
+    t_run_stream = P->run_stream;            // MS_EMUL_STREAMS at a __syncthreads() of this launch
+    t_run_kern = P->run_kern;
+    while (P->block[me] >= 0) {
+      tls.bdim = dim3{P->nthreads, 1, 1};
+      tls.gdim = dim3{P->grid, 1, 1};
+      tls.bid = uint3{(unsigned)P->block[me], 0, 0};
+      tls.tid = uint3{0, 0, 0};
+      in_cta_pool = true;
+      cta_switch(SW_START);                  // a CTA may start late
+      g_s->body = P->body;
+      memset(g_s->smem, 0xCD, P->dyn);
+      run_cta(g_s, P->nthreads);
+      g_s->body = nullptr;
+      in_cta_pool = false;
+      P->block[me] = P->next < P->grid ? (int)P->next++ : -1;
+    }
+    t_run_stream = nullptr;
+    t_run_kern = nullptr;
+    lk.lock();
+    int to = -1;                             // another resident CTA, else the launch is over
+    for (int w = 0; w < (int)P->block.size() && to < 0; w++)
+      if (P->block[w] >= 0) to = w;
+    P->turn = to;
+    P->cv.notify_all();
+  }
+  free_sched(g_top);
+  free_sched(g_nested);
+  g_s = g_top = g_nested = nullptr;
+}
+
+static bool ctas_launch(unsigned grid, unsigned block, size_t dyn, const std::function<void()>& body) {
+  if (grid < 2 || t_nested || !ctas_on()) return false;
+  const char* e = getenv("MS_EMUL_SMS");
+  const int sms = e ? atoi(e) : 1;
+  const unsigned resident = (unsigned)std::min(std::max(2 * sms, 2), 256);
+  if (!t_own_pool) { t_own_pool.reset(new CtaPool()); t_own_pool->owner = std::this_thread::get_id(); }
+  CtaPool* P = t_own_pool.get();
+  while (P->threads.size() < resident) {
+    P->block.push_back(-1);
+    P->hold.push_back(0);
+    P->threads.emplace_back(cta_worker, P, (int)P->threads.size());
+  }
+  P->body = &body;
+  P->grid = grid;
+  P->nthreads = block;
+  P->dyn = dyn;
+  P->run_stream = t_run_stream;
+  P->run_kern = t_run_kern;
+  P->passes = 0;
+  const unsigned first = std::min(grid, resident);
+  for (unsigned w = 0; w < P->block.size(); w++) { P->block[w] = w < first ? (int)w : -1; P->hold[w] = 0; }
+  P->next = first;
+  {
+    std::unique_lock<std::mutex> lk(P->mu);
+    P->turn = (int)(cta_rng(P) % first);
+    P->cv.notify_all();
+    P->cv.wait(lk, [&] { return P->turn == -1; });
+  }
+  std::lock_guard<std::mutex> g(g_cta_mu);
+  auto& c = g_cta_counts[t_kern];
+  c.first += P->passes ? 1 : 0;
+  c.second += P->passes;
+  return true;
+}
+
 }  // namespace simt
+
+// test hooks (tests/test_cta_interleave.py): switch the CTA mode at run time (-1: off), and per kernel (symbol
+// substring) the launches in which two CTAs overlapped and the baton passes from a CTA in mid-flight
+extern "C" void simt_ctas(long long seed) {
+  simt::g_cta_seed.store(seed < 0 ? -1 : seed);
+  simt::g_cta_gen++;
+}
+extern "C" void simt_cta_counts(const char* kern, unsigned long long* overlapped, unsigned long long* passes) {
+  std::lock_guard<std::mutex> g(simt::g_cta_mu);
+  *overlapped = *passes = 0;
+  for (const auto& kv : simt::g_cta_counts) {
+    Dl_info a{};
+    if (!dladdr(kv.first, &a) || !a.dli_sname || !strstr(a.dli_sname, kern)) continue;
+    *overlapped += kv.second.first;
+    *passes += kv.second.second;
+  }
+}
+extern "C" void simt_cta_counts_reset() {
+  std::lock_guard<std::mutex> g(simt::g_cta_mu);
+  simt::g_cta_counts.clear();
+}
 
 // test hooks (tests/test_stream_overlap.py): switch the stream mode at run time, and count the kernels that
 // ran while a top-level CTA was parked, by (parked kernel, kernel) symbol substrings
