@@ -46,7 +46,6 @@ constexpr uint64_t RECV_BIT = 1ull << 63;
 constexpr uint32_t kResolvedTicket = 0xFFFFFFu;   // order key of a record that carries its dense id: (id >> 32, this, id & 0xFFFFFFFF)
 
 // ------------------------------------------------------------------ small PTX helpers
-__device__ __forceinline__ uint32_t ld_cg_u32(const uint32_t* p) { return __ldcg(p); }
 // streaming 16-byte store: journal / ring records are written once and read by
 // another SM (or the host) later, so keep them out of L1.
 __device__ __forceinline__ void st_v4(uint4* p, uint4 v) {
@@ -182,6 +181,22 @@ __device__ __forceinline__ Rec win_rec(const Params& p, const Win& w, uint32_t e
   return rec_unpack(a, b, c);
 }
 
+// k_round's dynamic shared memory, `cap` = window capacity of the size class (25 B / message):
+//   reg1 u64[cap+1]  order keys (round << 24 | ticket)  ->  packed count scan
+//   keyB u32[cap]    emission index of the key
+//   vals u32[cap]    value | V_* flags        tab u16[2*cap]  first-sight table
+//   meta u16[cap]    compact message class
+//   ord  u16[cap]    sorted position -> window slot      blk u8[cap]  sorted position -> sender block
+struct RoundSmem {
+  uint64_t* reg1;
+  uint32_t* keyB;
+  uint32_t* vals;
+  uint16_t* tab;
+  uint16_t* meta;
+  uint16_t* ord;
+  uint8_t* blk;
+};
+
 // dense id of (round, ticket, idx): id_base[round] + emit_prefix[round][ticket] + idx
 __device__ __forceinline__ uint64_t dense_base(const Params& p, DevState* st, uint64_t round, uint32_t ticket) {
   if (ticket == kResolvedTicket) return round << 32;   // the record already carries its id (k_release)
@@ -195,13 +210,9 @@ __device__ __forceinline__ uint64_t dense_base(const Params& p, DevState* st, ui
 }
 
 // ------------------------------------------------------------------ block primitives
-// Exclusive scan of a[0..n) in shared memory, total written to a[n] and returned.
-__device__ uint64_t block_excl_scan(uint64_t* a, int n, uint64_t* wtmp /* >= 33 */) {
-  const int nt = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int c = (n + nt - 1) / nt;
-  const int lo = min(tid * c, n), hi = min(lo + c, n);
-  uint64_t sum = 0;
-  for (int i = lo; i < hi; i++) sum += a[i];
+// Exclusive prefix over the CTA of one u64 per thread (`sum`): a warp scan, then warp 0 scans the warp totals.
+// The CTA total is left in wtmp[32].
+__device__ __forceinline__ uint64_t cta_excl_scan_u64(uint64_t sum, int nt, int lane, int warp, uint64_t* wtmp /* >= 33 */) {
   uint64_t incl = sum;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
@@ -223,7 +234,17 @@ __device__ uint64_t block_excl_scan(uint64_t* a, int n, uint64_t* wtmp /* >= 33 
     if (lane == 31) wtmp[32] = wi;
   }
   __syncthreads();
-  uint64_t run = wtmp[warp] + incl - sum;
+  return wtmp[warp] + incl - sum;
+}
+
+// Exclusive scan of a[0..n) in shared memory, total written to a[n] and returned.
+__device__ uint64_t block_excl_scan(uint64_t* a, int n, uint64_t* wtmp /* >= 33 */) {
+  const int nt = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int c = (n + nt - 1) / nt;
+  const int lo = min(tid * c, n), hi = min(lo + c, n);
+  uint64_t sum = 0;
+  for (int i = lo; i < hi; i++) sum += a[i];
+  uint64_t run = cta_excl_scan_u64(sum, nt, lane, warp, wtmp);
   for (int i = lo; i < hi; i++) {
     const uint64_t v = a[i];
     a[i] = run;
@@ -282,6 +303,13 @@ __device__ __forceinline__ void journal_raw(const Params& p, uint64_t pos, uint6
     st_v4(b + 0, make_uint4((uint32_t)v, (uint32_t)(v >> 32), r.msg_id, r.in_reply_to));
     st_v4(b + 1, make_uint4(r.tf, r.p0, (uint32_t)r.p1, (uint32_t)(r.p1 >> 32)));
   }
+}
+
+// Claim of n raw journal positions for `ticket`'s chunk; the host has to have drained what they overwrite.
+__device__ __forceinline__ void journal_claim(const Params& p, DevState* st, uint32_t n, uint32_t ticket, uint64_t& chunk) {
+  chunk = (n && p.jlevel) ? atomicAdd((unsigned long long*)&st->jraw_cursor, (unsigned long long)n) : 0ull;
+  if (n && p.jlevel && !p.jdiscard && chunk + n - st->jraw_drained > p.jmask + 1)
+    latch_error(st, E_JOURNAL_OVERFLOW, ticket);
 }
 
 // ------------------------------------------------------------------ timing wheel (pooled chains)
@@ -549,9 +577,21 @@ __device__ __forceinline__ uint32_t class_of(const Params& p, uint32_t n) {
   return c;
 }
 
+// Entry li of a class's work list: its `big` longer windows are filled in from the front, the others from the back.
+__device__ __forceinline__ uint32_t list_ticket(const uint32_t* list, uint32_t big, uint32_t t_max, uint32_t li) {
+  return li < big ? list[li] : list[t_max - 1u - (li - big)];
+}
+
 // The per-endpoint part of k_snapshot for the threads gid, gid + stride, ...: also run by the single CTA of
 // k_glue (sharded runs), right after it has committed the previous round.
 __device__ void snapshot_endpoints(const Params& p, DevState* st, uint32_t gid, uint32_t stride);
+
+// One thread, after the snapshot: clears the class counters of the other parity (`par` = this round's) for the
+// next round and opens this round to k_round.
+__device__ __forceinline__ void open_round(DevState* st, uint32_t par) {
+  for (int c = 0; c < 4; c++) { st->cls_count[par ^ 1u][c] = 0; st->cls_small[par ^ 1u][c] = 0; st->cls_cursor[par ^ 1u][c] = 0; }
+  st->slot_open = slot_tag(st->round);
+}
 
 __global__ void k_snapshot(Params p) {
   DevState* st = p.st;
@@ -582,10 +622,7 @@ __global__ void k_snapshot(Params p) {
       if (threadIdx.x == 0) st->cal_ret_n = 0;
     }
   }
-  if (gid == 0) {
-    for (int c = 0; c < 4; c++) { st->cls_count[par ^ 1u][c] = 0; st->cls_small[par ^ 1u][c] = 0; st->cls_cursor[par ^ 1u][c] = 0; }
-    st->slot_open = slot_tag(st->round);
-  }
+  if (gid == 0) open_round(st, par);
 }
 
 __device__ void snapshot_endpoints(const Params& p, DevState* st, uint32_t gid, uint32_t stride) {
@@ -722,13 +759,6 @@ struct MsgView {
   uint32_t tf;   // type | flags << 16
 };
 
-__device__ __forceinline__ MsgView view_load(const uint4* rec) {
-  const uint4 b = rec[1], c = rec[2];
-  MsgView v;
-  v.src = b.x; v.msg_id = b.z; v.tf = c.x; v.p0 = c.y;
-  return v;
-}
-
 // vals[] bits
 constexpr uint32_t V_FRESH = 1u << 31;  // broadcast value unseen so far (after PC: first sight = new)
 constexpr uint32_t V_RECV = 1u << 30;   // passed the partition check
@@ -761,35 +791,11 @@ __device__ __forceinline__ uint32_t nbr_pos(const Params& p, uint32_t e, uint32_
   return 0xFFFFFFFFu;
 }
 
-// number of emissions of one delivered message (count phase)
+// position of `src` in e's neighbor list L, or 0xFFFFFFFF
 __device__ __forceinline__ uint32_t nbr_pos_l(const Params& p, uint32_t e, uint32_t src, const NbrList& L) {
   if (L.nl == nullptr) return nbr_pos(p, e, src);
   for (uint32_t j = 0; j < L.deg; j++) if (L.nl[j] == src) return j;
   return 0xFFFFFFFFu;
-}
-
-__device__ __forceinline__ uint32_t node_emit_count(const Params& p, uint32_t e, const MsgView& w, bool is_new,
-                                                    const NbrList& L) {
-  const uint32_t type = w.tf & 0xFFFFu;
-  const bool has_id = (w.tf >> 16) & MS_F_MSG_ID;
-  const bool is_reply = (w.tf >> 16) & MS_F_REPLY;
-  if (p.workload == MS_W_ECHO) {                       // demo/ruby/echo.rb:28-39
-    return (type == MS_T_INIT || type == MS_T_ECHO) ? 1u : 0u;
-  }
-  // broadcast node (doc/03-broadcast/01-broadcast.md:527-544, 02-performance.md:61-67)
-  if (is_reply) return 0;                              // node.rb:159-164
-  switch (type) {
-    case MS_T_INIT: case MS_T_TOPOLOGY: case MS_T_READ: return 1;
-    case MS_T_BROADCAST: {
-      uint32_t n = has_id ? 1u : 0u;
-      if (is_new) {
-        n += L.deg;
-        if (nbr_pos_l(p, e, w.src, L) != 0xFFFFFFFFu) n -= 1;   // skip whoever sent it to us
-      }
-      return n;
-    }
-    default: return has_id ? 1u : 0u;                  // error 10 not-supported (errors.edn)
-  }
 }
 
 // k-th emission of a delivered message (emit phase).  Returns the neighbor slot
@@ -987,11 +993,7 @@ __global__ void __launch_bounds__(512) k_glue(Params p, uint32_t open_next) {
   if (!round_skipped(p, st)) {                         // the state the commit has just left behind
     snapshot_endpoints(p, st, threadIdx.x, blockDim.x);
     __syncthreads();
-    if (threadIdx.x == 0) {
-      const uint32_t par = (uint32_t)st->round & 1u;
-      for (int c = 0; c < 4; c++) { st->cls_count[par ^ 1u][c] = 0; st->cls_small[par ^ 1u][c] = 0; st->cls_cursor[par ^ 1u][c] = 0; }
-      st->slot_open = slot_tag(st->round);
-    }
+    if (threadIdx.x == 0) open_round(st, (uint32_t)st->round & 1u);
   }
   barrier_body(p, &s_epoch);
 }
@@ -1055,34 +1057,13 @@ __global__ void __launch_bounds__(512) k_commit_b(Params p, uint32_t nb) {
     if (threadIdx.x == 0) p.cm_flags[2] = 0;
     return;
   }
-  // exclusive scan of the block sums in place (block_excl_scan wants shared memory: do it by hand)
+  // exclusive scan of the block sums in place (block_excl_scan wants shared memory)
   const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5;
   const int c = ((int)nb + nt - 1) / nt;
   const int lo = min(tid * c, (int)nb), hi = min(lo + c, (int)nb);
   uint64_t sum = 0;
   for (int i = lo; i < hi; i++) sum += p.cm_blk[i];
-  uint64_t incl = sum;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint64_t y = __shfl_up_sync(FULL, incl, d);
-    if (lane >= d) incl += y;
-  }
-  if (lane == 31) s_wtmp[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    const int nw = nt >> 5;
-    const uint64_t w = lane < nw ? s_wtmp[lane] : 0;
-    uint64_t wi = w;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint64_t y = __shfl_up_sync(FULL, wi, d);
-      if (lane >= d) wi += y;
-    }
-    s_wtmp[lane] = wi - w;
-    if (lane == 31) s_wtmp[32] = wi;
-  }
-  __syncthreads();
-  uint64_t run = s_wtmp[warp] + incl - sum;
+  uint64_t run = cta_excl_scan_u64(sum, nt, lane, warp, s_wtmp);
   for (int i = lo; i < hi; i++) {
     const uint64_t v = p.cm_blk[i];
     p.cm_blk[i] = run;
@@ -1141,13 +1122,7 @@ __global__ void __launch_bounds__(256) k_commit_c(Params p) {
 
 // ------------------------------------------------------------------ k_round
 // Persistent CTAs; one ticket at a time: tickets [0, n_inj_tickets) are injector
-// slices, ticket n_inj_tickets + e is endpoint e.  Dynamic shared memory, `cap` =
-// window capacity of this size class (25 B / message):
-//   reg1 u64[cap+1]  order keys (round << 24 | ticket)  ->  packed count scan
-//   keyB u32[cap]    emission index of the key
-//   vals u32[cap]    value | V_* flags        tab u16[2*cap]  first-sight table
-//   meta u16[cap]    compact message class
-//   ord  u16[cap]    sorted position -> window slot      blk u8[cap]  sorted position -> sender block
+// slices, ticket n_inj_tickets + e is endpoint e.  Dynamic shared memory: RoundSmem.
 constexpr uint32_t M_SRCSLOT = 0xFu;      // meta bits 0-3: neighbor slot of src + 1, 15 = neighbor (slot unknown), 0 = none
 constexpr uint32_t M_HAS_ID = 1u << 4;
 constexpr uint32_t M_REPLY = 1u << 5;
@@ -1165,42 +1140,22 @@ __device__ __forceinline__ uint32_t emit_count_meta(uint32_t workload, uint32_t 
   return has_id;                                                                         // error 10
 }
 
-// exclusive prefix of one u32 per thread over the CTA; total returned through *total
-__device__ __forceinline__ uint32_t block_excl_scan_u32(uint32_t v, uint32_t* total, uint32_t* wcnt /* >= 17 */) {
+// exclusive prefix of one value per thread over the CTA (u32, or u64 such as packed 4 x 16-bit counters): every
+// thread sums the warp totals itself; the CTA total is returned through *total
+template <typename T>
+__device__ __forceinline__ T block_excl_scan_v(T v, T* total, T* wtmp /* >= 17 */) {
   const int nt = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  uint32_t incl = v;
+  T incl = v;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t y = __shfl_up_sync(FULL, incl, d);
-    if (lane >= d) incl += y;
-  }
-  if (lane == 31) wcnt[warp] = incl;
-  __syncthreads();
-  uint32_t before = 0, tot = 0;
-  for (int w = 0; w < (nt >> 5); w++) {
-    const uint32_t cw = wcnt[w];
-    if (w < warp) before += cw;
-    tot += cw;
-  }
-  __syncthreads();
-  *total = tot;
-  return before + incl - v;
-}
-
-// same for one u64 per thread (packed 4 x 16-bit counters)
-__device__ __forceinline__ uint64_t block_excl_scan_u64v(uint64_t v, uint64_t* total, uint64_t* wtmp /* >= 17 */) {
-  const int nt = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  uint64_t incl = v;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint64_t y = __shfl_up_sync(FULL, incl, d);
+    const T y = __shfl_up_sync(FULL, incl, d);
     if (lane >= d) incl += y;
   }
   if (lane == 31) wtmp[warp] = incl;
   __syncthreads();
-  uint64_t before = 0, tot = 0;
+  T before = 0, tot = 0;
   for (int w = 0; w < (nt >> 5); w++) {
-    const uint64_t cw = wtmp[w];
+    const T cw = wtmp[w];
     if (w < warp) before += cw;
     tot += cw;
   }
@@ -1223,7 +1178,7 @@ __device__ __forceinline__ uint32_t gset_emit_count(uint32_t meta) {
 // sum of one u32 per thread over the CTA
 __device__ __forceinline__ uint32_t block_sum_u32(uint32_t v, uint32_t* wcnt /* >= 17 */) {
   uint32_t total;
-  (void)block_excl_scan_u32(v, &total, wcnt);
+  (void)block_excl_scan_v(v, &total, wcnt);
   return total;
 }
 
@@ -1323,6 +1278,93 @@ __device__ void service_handle(const Params& p, uint32_t svc, const SvReq& q, ui
   }
 }
 
+// ------------------------------------------------------------------ node programs run by k_round
+// Raft / txn-list-append server e (ms_raft.cuh), one thread: the window in id order, then the node's timers.
+// Returns the number of sends it staged in rf_stage; k_round emits them.
+__device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const Win& w,
+                              uint32_t n, const RoundSmem& sm) {
+  RaftCtx c{p, st, e, now, round, p.rf_node + e, p.rf_log + (size_t)e * p.rf_log_cap * 2,
+            p.rf_cb + (size_t)e * (p.rf_cb_mask + 1u) * 2, p.rf_stage + (size_t)e * p.rf_stage_cap * 3, 0u, 0u, 0u, 0u};
+  rf_group_of(p, e, c.gbase, c.gn);
+  for (uint32_t pos = 0; pos < n; pos++) {
+    const uint32_t i = sm.ord[pos];
+    if (!(sm.vals[i] & V_RECV)) continue;
+    const uint4* rp = w.ring + (size_t)((w.head + i) & w.mask) * 3;
+    if (p.workload == MS_W_RAFT) rf_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+    else if (p.workload == MS_W_TXN_TREE) tt_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+    else txn_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+  }
+  if (p.workload == MS_W_RAFT) { rf_actions(c); rf_note_busy(c); }
+  if (p.workload == MS_W_TXN_TREE) tt_actions(c);
+  return c.n_stage;
+}
+
+// Service endpoint e: requests are handled one at a time in dequeue order (service.clj:147-156, 245-263) by one
+// thread; the reply is parked in vals[] / keyB[] for the emit phase.  Called by the whole CTA.
+__device__ void sv_step(const Params& p, DevState* st, uint32_t e, uint64_t round, const Win& w, uint32_t n,
+                        const RoundSmem& sm) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  // the request fields the sequential walk needs, staged in sorted order by all threads (the
+  // ordering keys are dead by now): p1 in reg1, the key in tab (as u32), type | flags << 8 in meta
+  uint32_t* skey = reinterpret_cast<uint32_t*>(sm.tab);
+  for (uint32_t pos = tid; pos < n; pos += nt) {
+    const uint32_t i = sm.ord[pos];
+    const uint4* rp = w.ring + (size_t)((w.head + i) & w.mask) * 3;
+    const uint4 vc = rp[2];
+    sm.reg1[pos] = (uint64_t)vc.z | ((uint64_t)vc.w << 32);
+    skey[pos] = vc.y;
+    const uint32_t ty = vc.x & 0xFFFFu;                       // types the device does not know (>= 256) stay unknown
+    sm.meta[i] = (uint16_t)((ty < 0xFFu ? ty : 0xFFu) | ((vc.x >> 8) & 0xFF00u));
+  }
+  __syncthreads();
+  if (tid == 0) {
+    uint32_t svc = 0;
+    while (svc < 4 && p.sv_ep[svc] != e) svc++;
+    uint32_t n_rep = 0;
+    // lin-kv: the binding of the key last touched stays in registers (single_key_txn.clj has every
+    // node hammer ONE key, the root): the walk is a dependent chain, keep memory out of it
+    uint32_t ck = 0xFFFFFFFFu, cval = 0;
+    bool chas = false, cdirty = false;
+    for (uint32_t pos = 0; pos < n && svc < 4; pos++) {
+      const uint32_t i = sm.ord[pos];
+      if (!(sm.vals[i] & V_RECV)) continue;
+      SvReq q;
+      q.type = sm.meta[i] & 0xFFu; q.flags = sm.meta[i] >> 8; q.key = skey[pos];
+      q.p1 = sm.reg1[pos];
+      q.src = 0;
+      if (svc == MS_SVC_SEQ_KV)                               // per-client view (service.clj:162-166)
+        q.src = (w.ring + (size_t)((w.head + i) & w.mask) * 3)[1].x;
+      const bool keyed = q.type == MS_T_READ || q.type == MS_T_WRITE || q.type == MS_T_CAS;
+      if (svc != MS_SVC_LIN_TSO && keyed && q.key >= p.sv_n_keys) { latch_error(st, E_VALUE_RANGE, q.key); continue; }
+      if (svc != MS_SVC_LIN_TSO && !keyed) continue;   // no clause of the store's `case` matches: logged, no reply (service.clj:262-263)
+      uint32_t x[4] = {0, 0, 0, 0};
+      if (svc == MS_SVC_SEQ_KV || svc == MS_SVC_LWW_KV)      // rand-int = word 3 of the reply's own draw
+        philox4x32_10(n_rep, e, (uint32_t)round, (uint32_t)(round >> 32), p.seed_lo, p.seed_hi, x);
+      SvRep r;
+      if (svc == MS_SVC_LIN_KV) {
+        r.reply = false; r.otype = MS_T_ERROR; r.code = 0; r.value = 0;
+        if (keyed) {
+          if (q.key != ck) {
+            if (cdirty) { p.sv_lin_has[ck] = chas ? 1 : 0; p.sv_lin_val[ck] = cval; }
+            ck = q.key; chas = p.sv_lin_has[ck] != 0; cval = p.sv_lin_val[ck]; cdirty = false;
+          }
+          bool np_; uint32_t nv;
+          kv_eval(chas, cval, q, false, r, np_, nv);
+          if (r.reply) { cdirty = cdirty || np_ != chas || nv != cval; chas = np_; cval = nv; }
+        }
+      } else {
+        service_handle(p, svc, q, x[3], r);
+      }
+      if (r.reply) {
+        sm.vals[i] |= SV_REPLY | (r.code << 16) | r.otype;
+        sm.keyB[pos] = r.value;
+        n_rep++;
+      }
+    }
+    if (cdirty) { p.sv_lin_has[ck] = chas ? 1 : 0; p.sv_lin_val[ck] = cval; }
+  }
+  __syncthreads();
+}
 
 // WL = node-program families compiled in: bit 0 g-set, bit 2 Raft (else echo / broadcast), bit 1 services.
 // CTA width per window-size class (ms_engine.cu: 64 / 128 / 256 / 512 threads; the g-set family runs
@@ -1360,6 +1402,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
   uint16_t* meta = tab + 2 * (size_t)cap;
   uint16_t* ord = meta + cap;
   uint8_t* blk = reinterpret_cast<uint8_t*>(ord + cap);
+  const RoundSmem sm{reg1, keyB, vals, tab, meta, ord, blk};
   uint64_t* keyA = reg1;
   uint64_t* aux = reg1;                                            // packed counts (keyA is dead by then)
 
@@ -1442,7 +1485,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
   // fetch the index of the NEXT ticket now; it is consumed at the end of this one
   uint32_t next_li = 0;
   if (tid == 0) next_li = atomicAdd(&st->cls_cursor[par][cls], 1u);
-  const uint32_t ticket = li < my_big ? my_list[li] : my_list[p.t_max - 1u - (li - my_big)];
+  const uint32_t ticket = list_ticket(my_list, my_big, p.t_max, li);
   PHASE_MARK(0);
   if (timing && tid == 0) atomicAdd((unsigned long long*)&p.phase_cycles[cls * 16 + 15], 1ull);
 
@@ -1474,12 +1517,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     const uint32_t lo = min(ticket * chunk, K), hi_s = min(lo + chunk, K);
     const uint32_t n_local = hi_s - lo;
     n_ev_local = n_local; n_em_local = n_local;
-    if (tid == 0) {
-      s_chunk = (n_local && p.jlevel)
-                    ? atomicAdd((unsigned long long*)&st->jraw_cursor, (unsigned long long)n_local) : 0ull;
-      if (n_local && p.jlevel && !p.jdiscard && s_chunk + n_local - st->jraw_drained > p.jmask + 1)
-        latch_error(st, E_JOURNAL_OVERFLOW, ticket);
-    }
+    if (tid == 0) journal_claim(p, st, n_local, ticket, s_chunk);
     __syncthreads();
     cx.chunk = s_chunk;
     cx.emitter = kInjector;
@@ -1645,7 +1683,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     // this CTA's NEXT ticket: pull its window from HBM into L2 now, behind this ticket's remaining phases
     // (windows are frozen by k_snapshot, so head / limit are final; a window is contiguous up to the ring's wrap)
     if (tid == 0 && next_li < my_count) {
-      const uint32_t t2 = next_li < my_big ? my_list[next_li] : my_list[p.t_max - 1u - (next_li - my_big)];
+      const uint32_t t2 = list_ticket(my_list, my_big, p.t_max, next_li);
       if (t2 >= p.n_inj_tickets) {
         const uint32_t e2 = t2 - p.n_inj_tickets;
         const uint32_t h2 = p.head[e2], n2 = p.limit[e2] - h2, cap2 = ring_cap_of(p, e2);
@@ -1693,7 +1731,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
           pa = ka; pb = kb;
         }
       }
-      uint32_t off = block_excl_scan_u32(nf, &R, s_wcnt);
+      uint32_t off = block_excl_scan_v(nf, &R, s_wcnt);
       if (R <= MAXB) {
         if (use_mask) {
           while (fmask) { s_bstart[off++] = (uint16_t)(lo + __ffs(fmask) - 1); fmask &= fmask - 1u; }
@@ -1823,24 +1861,9 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       __syncthreads();
     }
     if constexpr (RF) {
-      // ---- Raft / txn-list-append node: the step is sequential (ms_raft.cuh); its sends are staged and emitted below
+      // ---- Raft / txn-list-append node: its sends are staged and emitted below
       if (is_server) {
-        if (tid == 0) {
-          RaftCtx c{p, st, e, now, round, p.rf_node + e, p.rf_log + (size_t)e * p.rf_log_cap * 2,
-                    p.rf_cb + (size_t)e * (p.rf_cb_mask + 1u) * 2, p.rf_stage + (size_t)e * p.rf_stage_cap * 3, 0u, 0u, 0u, 0u};
-          rf_group_of(p, e, c.gbase, c.gn);
-          for (uint32_t pos = 0; pos < n; pos++) {
-            const uint32_t i = ord[pos];
-            if (!(vals[i] & V_RECV)) continue;
-            const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
-            if (p.workload == MS_W_RAFT) rf_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
-            else if (p.workload == MS_W_TXN_TREE) tt_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
-            else txn_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
-          }
-          if (p.workload == MS_W_RAFT) { rf_actions(c); rf_note_busy(c); }
-          if (p.workload == MS_W_TXN_TREE) tt_actions(c);
-          s_misc[2] = c.n_stage;
-        }
+        if (tid == 0) s_misc[2] = raft_step(p, st, e, now, round, win, n, sm);
         __syncthreads();
         n_timer = s_misc[2];
       }
@@ -1860,70 +1883,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       n_timer = s_misc[2];
     }
     if constexpr (SV) {
-      // ---- service endpoint: requests are handled one at a time in dequeue order (service.clj:147-156,
-      //      245-263) by one thread; the reply is parked in vals[] / keyB[] for the emit phase
-      if (kind == MS_KIND_SERVICE) {
-        // the request fields the sequential walk needs, staged in sorted order by all threads (the
-        // ordering keys are dead by now): p1 in reg1, the key in tab (as u32), type | flags << 8 in meta
-        uint32_t* skey = reinterpret_cast<uint32_t*>(tab);
-        for (uint32_t pos = tid; pos < n; pos += nt) {
-          const uint32_t i = ord[pos];
-          const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
-          const uint4 vc = rp[2];
-          reg1[pos] = (uint64_t)vc.z | ((uint64_t)vc.w << 32);
-          skey[pos] = vc.y;
-          const uint32_t ty = vc.x & 0xFFFFu;                       // types the device does not know (>= 256) stay unknown
-          meta[i] = (uint16_t)((ty < 0xFFu ? ty : 0xFFu) | ((vc.x >> 8) & 0xFF00u));
-        }
-        __syncthreads();
-        if (tid == 0) {
-          uint32_t svc = 0;
-          while (svc < 4 && p.sv_ep[svc] != e) svc++;
-          uint32_t n_rep = 0;
-          // lin-kv: the binding of the key last touched stays in registers (single_key_txn.clj has every
-          // node hammer ONE key, the root): the walk is a dependent chain, keep memory out of it
-          uint32_t ck = 0xFFFFFFFFu, cval = 0;
-          bool chas = false, cdirty = false;
-          for (uint32_t pos = 0; pos < n && svc < 4; pos++) {
-            const uint32_t i = ord[pos];
-            if (!(vals[i] & V_RECV)) continue;
-            SvReq q;
-            q.type = meta[i] & 0xFFu; q.flags = meta[i] >> 8; q.key = skey[pos];
-            q.p1 = reg1[pos];
-            q.src = 0;
-            if (svc == MS_SVC_SEQ_KV)                               // per-client view (service.clj:162-166)
-              q.src = (myring + (size_t)((head + i) & my_mask) * 3)[1].x;
-            const bool keyed = q.type == MS_T_READ || q.type == MS_T_WRITE || q.type == MS_T_CAS;
-            if (svc != MS_SVC_LIN_TSO && keyed && q.key >= p.sv_n_keys) { latch_error(st, E_VALUE_RANGE, q.key); continue; }
-            if (svc != MS_SVC_LIN_TSO && !keyed) continue;   // no clause of the store's `case` matches: logged, no reply (service.clj:262-263)
-            uint32_t x[4] = {0, 0, 0, 0};
-            if (svc == MS_SVC_SEQ_KV || svc == MS_SVC_LWW_KV)      // rand-int = word 3 of the reply's own draw
-              philox4x32_10(n_rep, e, (uint32_t)round, (uint32_t)(round >> 32), p.seed_lo, p.seed_hi, x);
-            SvRep r;
-            if (svc == MS_SVC_LIN_KV) {
-              r.reply = false; r.otype = MS_T_ERROR; r.code = 0; r.value = 0;
-              if (keyed) {
-                if (q.key != ck) {
-                  if (cdirty) { p.sv_lin_has[ck] = chas ? 1 : 0; p.sv_lin_val[ck] = cval; }
-                  ck = q.key; chas = p.sv_lin_has[ck] != 0; cval = p.sv_lin_val[ck]; cdirty = false;
-                }
-                bool np_; uint32_t nv;
-                kv_eval(chas, cval, q, false, r, np_, nv);
-                if (r.reply) { cdirty = cdirty || np_ != chas || nv != cval; chas = np_; cval = nv; }
-              }
-            } else {
-              service_handle(p, svc, q, x[3], r);
-            }
-            if (r.reply) {
-              vals[i] |= SV_REPLY | (r.code << 16) | r.otype;
-              keyB[pos] = r.value;
-              n_rep++;
-            }
-          }
-          if (cdirty) { p.sv_lin_has[ck] = chas ? 1 : 0; p.sv_lin_val[ck] = cval; }
-        }
-        __syncthreads();
-      }
+      if (kind == MS_KIND_SERVICE) sv_step(p, st, e, round, win, n, sm);
     }
     // resolve winners and publish packed counts in sorted order:
     //   emit (bits 0-31) | recv (32-47) | new (48-63)
@@ -2071,7 +2031,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         const uint32_t ss = meta[i] & M_SRCSLOT;
         if ((vals[i] & V_FRESH) && ss >= 1 && ss <= 4) acc += 1ull << (16 * (ss - 1));
       }
-      uint64_t run = block_excl_scan_u64v(acc, &f_total, s_wtmp);
+      uint64_t run = block_excl_scan_v(acc, &f_total, s_wtmp);
       for (int pos = lo; pos < hi; pos++) {
         const uint32_t i = ord[pos];
         const uint32_t ss = meta[i] & M_SRCSLOT;
@@ -2083,10 +2043,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     if (timing && tid == 0 && bcast && n_new > 0) atomicAdd((unsigned long long*)&p.phase_cycles[cls * 16 + (agg ? 11 : 12)], 1ull);
     if (timing && tid == 0 && n > 1) atomicAdd((unsigned long long*)&p.phase_cycles[cls * 16 + 13], (unsigned long long)R);
     if (tid == 32 % nt) {
-      s_chunk = (n_ev_local && p.jlevel)
-                    ? atomicAdd((unsigned long long*)&st->jraw_cursor, (unsigned long long)n_ev_local) : 0ull;
-      if (n_ev_local && p.jlevel && !p.jdiscard && s_chunk + n_ev_local - st->jraw_drained > p.jmask + 1)
-        latch_error(st, E_JOURNAL_OVERFLOW, ticket);
+      journal_claim(p, st, n_ev_local, ticket, s_chunk);
       if (mailed && n_recv) s_misc[0] = atomicAdd(&st->mail_count, n_recv);
     }
     if (agg && tid < (int)deg) {   // deg <= MAXNB <= 32 <= blockDim
@@ -2357,6 +2314,49 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
 #undef TAB_SLOT
 }
 
+// ------------------------------------------------------------------ journal chunks
+// The raw journal chunk of one (round, ticket): its events are g0 .. g0 + cnt - 1 at raw positions chunk + k; a
+// :send's id is send_base + its raw value.
+struct JChunk {
+  const RoundMeta* m;
+  uint64_t g0, cnt, chunk, send_base;
+};
+// Chunk c = (r - r0) * t_max + ticket of the rounds from r0 on: false when the round is not in the history, the
+// ticket did not run, runs on another shard, or has no events in [first, first + count).
+__device__ __forceinline__ bool journal_chunk(const Params& p, uint64_t r0, uint64_t c, uint64_t first, uint64_t count,
+                                              JChunk& j) {
+  const uint64_t r = r0 + c / p.t_max;
+  const uint32_t t = (uint32_t)(c % p.t_max);
+  const uint32_t row = (uint32_t)r & p.hist_mask;
+  const RoundMeta* m = p.rmeta + row;
+  if (m->round != r || t >= m->n_tickets) return false;
+  if (owner_of_ticket(t, p.n_inj_tickets, p.n_servers, p.n_shards) != p.shard_id) return false;   // chunk lives on another shard
+  const uint32_t* ev = p.rt_ev + (size_t)row * p.t_max;
+  const uint64_t off = ev[t];
+  const uint64_t end = (t + 1 < m->n_tickets) ? ev[t + 1] : m->ev_total;
+  if (end == off) return false;
+  const uint64_t g0 = m->ev_base + off;
+  const uint64_t cnt = end - off;
+  if (g0 + cnt <= first || g0 >= first + count) return false;
+  j = JChunk{m, g0, cnt, p.rt_chunk[(size_t)row * p.t_max + t], m->id_base + p.rt_em[(size_t)row * p.t_max + t]};
+  return true;
+}
+
+// 32-byte event record of event g (MS_JFMT_EVENT): {event id | recv flag, time}, {message id, src, dest} (raw.z, raw.w)
+__device__ __forceinline__ void event_rec(uint64_t g, bool recv, int64_t tnow, uint64_t id, uint4 raw, uint4& a, uint4& b) {
+  const uint64_t eid = g | (recv ? MS_EVENT_RECV : 0ull);
+  a = make_uint4((uint32_t)eid, (uint32_t)(eid >> 32), (uint32_t)tnow, (uint32_t)((uint64_t)tnow >> 32));
+  b = make_uint4((uint32_t)id, (uint32_t)(id >> 32), raw.z, raw.w);
+}
+
+// MS_JFMT_8 word of an event: recv (1) | src (16) | dest (16) | id - id_ref (31); sets `bad` when a field does not fit
+__device__ __forceinline__ uint64_t jfmt8_word(uint64_t id, uint64_t id_ref, bool recv, uint4 raw, bool& bad) {
+  const uint64_t d = id - id_ref;
+  if (id < id_ref || d >= (1ull << 31) || raw.z > 0xFFFFu || raw.w > 0xFFFFu) bad = true;
+  return (recv ? RECV_BIT : 0ull) | ((uint64_t)(raw.z & 0xFFFFu) << 47) | ((uint64_t)(raw.w & 0xFFFFu) << 31) |
+         (d & 0x7FFFFFFFull);
+}
+
 // ------------------------------------------------------------------ k_journal_expand (K3)
 // Turns the raw per-(round, ticket) chunks of rounds [r0, r0 + n_rounds) into
 // journal events in event-id order (journal.clj:225-239) for the event window
@@ -2368,22 +2368,10 @@ __global__ void k_journal_expand(Params p, uint64_t r0, uint32_t n_rounds, uint6
   const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
   const uint64_t n_chunks = (uint64_t)n_rounds * p.t_max;
   for (uint64_t c = warp_global; c < n_chunks; c += n_warps) {
-    const uint64_t r = r0 + c / p.t_max;
-    const uint32_t t = (uint32_t)(c % p.t_max);
-    const uint32_t row = (uint32_t)r & p.hist_mask;
-    const RoundMeta* m = p.rmeta + row;
-    if (m->round != r || t >= m->n_tickets) continue;
-    if (owner_of_ticket(t, p.n_inj_tickets, p.n_servers, p.n_shards) != p.shard_id) continue;   // chunk lives on another shard
-    const uint32_t* ev = p.rt_ev + (size_t)row * p.t_max;
-    const uint64_t off = ev[t];
-    const uint64_t end = (t + 1 < m->n_tickets) ? ev[t + 1] : m->ev_total;
-    if (end == off) continue;
-    const uint64_t g0 = m->ev_base + off;
-    const uint64_t cnt = end - off;
-    if (g0 + cnt <= first || g0 >= first + count) continue;
-    const uint64_t chunk = p.rt_chunk[(size_t)row * p.t_max + t];
-    const uint64_t send_base = m->id_base + p.rt_em[(size_t)row * p.t_max + t];
-    const int64_t tnow = m->now;
+    JChunk j;
+    if (!journal_chunk(p, r0, c, first, count, j)) continue;
+    const uint64_t g0 = j.g0, cnt = j.cnt, chunk = j.chunk, send_base = j.send_base;
+    const int64_t tnow = j.m->now;
     for (uint64_t k = lane; k < cnt; k += 32) {
       const uint64_t g = g0 + k;
       if (g < first || g >= first + count) continue;
@@ -2391,10 +2379,11 @@ __global__ void k_journal_expand(Params p, uint64_t r0, uint32_t n_rounds, uint6
       const uint64_t v = (uint64_t)raw.x | ((uint64_t)raw.y << 32);
       const bool recv = (v & RECV_BIT) != 0;
       const uint64_t id = recv ? (v & ~RECV_BIT) : send_base + v;
-      const uint64_t eid = g | (recv ? MS_EVENT_RECV : 0ull);
+      uint4 e0, e1;
+      event_rec(g, recv, tnow, id, raw, e0, e1);
       uint4* o = out_ev + (g - first) * 2;
-      st_v4(o + 0, make_uint4((uint32_t)eid, (uint32_t)(eid >> 32), (uint32_t)tnow, (uint32_t)((uint64_t)tnow >> 32)));
-      st_v4(o + 1, make_uint4((uint32_t)id, (uint32_t)(id >> 32), raw.z, raw.w));
+      st_v4(o + 0, e0);
+      st_v4(o + 1, e1);
       if (out_body) {
         const uint4* b = p.jbody + ((chunk + k) & p.jmask) * 2;
         const uint4 b0 = b[0], b1 = b[1];
@@ -2484,21 +2473,10 @@ __global__ void k_journal_pack(Params p, StreamPlan* plan, unsigned char* out) {
   const uint64_t n_chunks = (uint64_t)n_rounds * p.t_max;
   bool bad = false;
   for (uint64_t c = warp_global; c < n_chunks; c += n_warps) {
-    const uint64_t r = r0 + c / p.t_max;
-    const uint32_t t = (uint32_t)(c % p.t_max);
-    const uint32_t row = (uint32_t)r & p.hist_mask;
-    const RoundMeta* m = p.rmeta + row;
-    if (m->round != r || t >= m->n_tickets) continue;
-    if (owner_of_ticket(t, p.n_inj_tickets, p.n_servers, p.n_shards) != p.shard_id) continue;
-    const uint32_t* ev = p.rt_ev + (size_t)row * p.t_max;
-    const uint64_t off = ev[t];
-    const uint64_t end = (t + 1 < m->n_tickets) ? ev[t + 1] : m->ev_total;
-    if (end == off) continue;
-    const uint64_t g0 = m->ev_base + off;
-    const uint64_t cnt = end - off;
-    if (g0 + cnt <= first || g0 >= first + count) continue;
-    const uint64_t chunk = p.rt_chunk[(size_t)row * p.t_max + t];
-    const uint64_t send_base = m->id_base + p.rt_em[(size_t)row * p.t_max + t];
+    JChunk j;
+    if (!journal_chunk(p, r0, c, first, count, j)) continue;
+    const RoundMeta* m = j.m;
+    const uint64_t g0 = j.g0, cnt = j.cnt, chunk = j.chunk, send_base = j.send_base;
     const uint64_t id_ref = m->id_base > (1ull << 30) ? m->id_base - (1ull << 30) : 0ull;
     const int64_t tnow = m->now;
     // sharded runs: a shard holds only its own endpoints' events, so the batch is not positional: the
@@ -2518,26 +2496,18 @@ __global__ void k_journal_pack(Params p, StreamPlan* plan, unsigned char* out) {
       const uint64_t id = recv ? (v & ~RECV_BIT) : send_base + v;
       if (p.n_shards > 1) {
         const uint64_t at = slot0 + (k - k_lo);
-        const uint64_t eid = g | (recv ? MS_EVENT_RECV : 0ull);
         if (FMT == 32) {
           uint4* o = reinterpret_cast<uint4*>(out) + at * 2;
-          o[0] = make_uint4((uint32_t)eid, (uint32_t)(eid >> 32), (uint32_t)tnow, (uint32_t)((uint64_t)tnow >> 32));
-          o[1] = make_uint4((uint32_t)id, (uint32_t)(id >> 32), raw.z, raw.w);
+          event_rec(g, recv, tnow, id, raw, o[0], o[1]);
         } else {                                             // MS_JFMT_16: event id word + the MS_JFMT_8 word
-          const uint64_t d = id - id_ref;
-          if (id < id_ref || d >= (1ull << 31) || raw.z > 0xFFFFu || raw.w > 0xFFFFu) bad = true;
-          const uint64_t w = (recv ? RECV_BIT : 0ull) | ((uint64_t)(raw.z & 0xFFFFu) << 47) |
-                             ((uint64_t)(raw.w & 0xFFFFu) << 31) | (d & 0x7FFFFFFFull);
+          const uint64_t eid = g | (recv ? MS_EVENT_RECV : 0ull);
+          const uint64_t w = jfmt8_word(id, id_ref, recv, raw, bad);
           reinterpret_cast<uint4*>(out)[at] = make_uint4((uint32_t)eid, (uint32_t)(eid >> 32), (uint32_t)w, (uint32_t)(w >> 32));
         }
         continue;
       }
       if (FMT == 8) {
-        const uint64_t d = id - id_ref;
-        if (id < id_ref || d >= (1ull << 31) || raw.z > 0xFFFFu || raw.w > 0xFFFFu) bad = true;
-        const uint64_t w = (recv ? RECV_BIT : 0ull) | ((uint64_t)(raw.z & 0xFFFFu) << 47) |
-                           ((uint64_t)(raw.w & 0xFFFFu) << 31) | (d & 0x7FFFFFFFull);
-        reinterpret_cast<unsigned long long*>(out)[g - first] = w;
+        reinterpret_cast<unsigned long long*>(out)[g - first] = jfmt8_word(id, id_ref, recv, raw, bad);
       } else if (FMT == 4) {
         // 32 bits per event.  A :send is {0, src (15), dest (16)}: sends appear in the journal in id order (both
         // counters are handed out in journal order, net.clj:197, journal.clj:228), so its id is implied by its
@@ -2559,10 +2529,8 @@ __global__ void k_journal_pack(Params p, StreamPlan* plan, unsigned char* out) {
         o[1] = (uint32_t)((id >> 32) & 0x7FFFu) | (recv ? 0x8000u : 0u) | ((raw.z & 0xFFFFu) << 16);
         o[2] = ((raw.z >> 16) & 0xFFu) | (raw.w << 8);
       } else {
-        const uint64_t eid = g | (recv ? MS_EVENT_RECV : 0ull);
         uint4* o = reinterpret_cast<uint4*>(out) + (g - first) * 2;
-        o[0] = make_uint4((uint32_t)eid, (uint32_t)(eid >> 32), (uint32_t)tnow, (uint32_t)((uint64_t)tnow >> 32));
-        o[1] = make_uint4((uint32_t)id, (uint32_t)(id >> 32), raw.z, raw.w);
+        event_rec(g, recv, tnow, id, raw, o[0], o[1]);
       }
     }
   }
