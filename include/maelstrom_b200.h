@@ -256,6 +256,43 @@ enum { MS_HF_BROADCAST = 0, MS_HF_READ = 1 };
 int ms_add_gen_clients(ms_sim* sim, const ms_gen_config* cfg, uint32_t first_name);
 int ms_history_drain(ms_sim* sim, ms_hist* out, size_t cap, size_t* n_out);
 
+/* Closed-loop lin-kv clients on the device (MS_W_RAFT): what a Jepsen worker does with the lin-kv client
+ * (workload/lin_kv.clj:40-76) and the generator of jepsen.tests.linearizable-register (lin_kv.clj:78-85).
+ * The client side is that of ms_add_gen_clients: one outstanding request, msg_id from 1, only in_reply_to is
+ * matched (the reply to a proxied request comes from the leader, raft.py:558-561), timeout, :ok / :fail /
+ * :info with reads idempotent (lin_kv.clj:52), stagger uniform on [0, 2 interval) from the client's own
+ * Philox stream (op, endpoint, 0xC11E47, 0): word 0 picks write / cas, word 1 the stagger, words 2 and 3 the
+ * values.  With g servers per Raft cluster (ms_config.reserved[4], 0 = all) and C = n_nodes / g whole clusters:
+ *   binding  client k is in group k / 2g, which works on cluster (k / 2g) mod C, and talks to server
+ *            cluster * g + k mod g (independent/concurrent-generator (* 2 n): 2n threads per key, thread i
+ *            on node i mod n); n_clients is a multiple of 2g
+ *   roles    (gen/reserve n r (gen/mix [w cas cas])): k mod 2g < g only reads; the others write with
+ *            probability 1/3, else cas
+ *   values   (rand-int 5): write value, cas from and to are (x * value_range) >> 32 of words 2 and 3
+ *   key      every client of a group works on key_base + (now / key_period_ns) mod keys_per_group, where
+ *            key_base = (group / C) * keys_per_group: the groups of one cluster have disjoint ranges, all below
+ *            ms_config.reserved[2] and 65536.  The reference moves a group on after a number of ops per key;
+ *            a function of virtual time needs no state shared between the clients of a round
+ *   messages MS_T_READ p0 = key; MS_T_WRITE p0 = key, p1 = value; MS_T_CAS p0 = key, p1 = from | to << 32
+ *   end      nothing is invoked at or after time_limit_ns (no quiet period, no final read); an op
+ *            outstanding then still completes or times out
+ *   history  ms_hist.f = MS_HF_KV_*, value = key | a << 16 | b << 24.  write: a = value; cas: a = from,
+ *            b = to; read: a = the value of the read_ok (invocations and failed reads carry the key only).
+ *            A read of a missing key is error 20, :fail (raft.py:169-173); errors 11 and 22 are :fail. */
+typedef struct ms_kv_gen_config {
+  uint32_t n_clients;        /* a multiple of 2g */
+  uint32_t value_range;      /* 0 = 5 (rand-int 5); <= 256 */
+  uint32_t keys_per_group;   /* >= 1 */
+  int64_t  interval_ns;      /* mean delay between two ops of one client */
+  int64_t  timeout_ns;       /* 0 = max(10 x ms_config.latency_mean_ms, 1000) ms (lin_kv.clj:54) */
+  int64_t  time_limit_ns;    /* --time-limit */
+  int64_t  key_period_ns;    /* > 0: virtual time a group spends on one key */
+} ms_kv_gen_config;
+enum { MS_HF_KV_READ = 2, MS_HF_KV_WRITE = 3, MS_HF_KV_CAS = 4 };
+/* adds cfg->n_clients endpoints "c<first_name> ..." and returns the index of the first.  MS_W_RAFT on one GPU,
+ * once per simulation, not together with ms_add_gen_clients; the history comes out of ms_history_drain */
+int ms_add_kv_clients(ms_sim* sim, const ms_kv_gen_config* cfg, uint32_t first_name);
+
 /* Upload a time-sorted schedule of client ops (appends). */
 int ms_schedule_ops(ms_sim* sim, const ms_op* ops, size_t n);
 

@@ -25,6 +25,7 @@ public final class Native {
   public static native long sendJson(long h, String line);
   public static native int recvJson(long h, int endpoint, long timeoutNs, ByteBuffer outUtf8, long cap);
   public static native int addGenClients(long h, ByteBuffer msGenConfig, int firstName);
+  public static native int addKvClients(long h, ByteBuffer msKvGenConfig, int firstName);
   public static native long historyDrain(long h, ByteBuffer msHist32, long cap);
   public static native int scheduleOps(long h, ByteBuffer msOps, long n);
   public static native int step(long h, long nRounds);

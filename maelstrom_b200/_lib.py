@@ -49,6 +49,12 @@ class GenConfig(C.Structure):   # ms_gen_config
                 ("timeout_ns", C.c_int64), ("time_limit_ns", C.c_int64), ("quiet_ns", C.c_int64)]
 
 
+class KvGenConfig(C.Structure):   # ms_kv_gen_config
+    _fields_ = [("n_clients", C.c_uint32), ("value_range", C.c_uint32), ("keys_per_group", C.c_uint32),
+                ("interval_ns", C.c_int64), ("timeout_ns", C.c_int64), ("time_limit_ns", C.c_int64),
+                ("key_period_ns", C.c_int64)]
+
+
 HIST_DTYPE = np.dtype([("time_ns", "<i8"), ("order", "<u8"), ("client", "<u4"), ("op", "<u4"), ("type", "u1"),
                        ("f", "u1"), ("error", "<u2"), ("value", "<u4")])
 assert HIST_DTYPE.itemsize == 32
@@ -82,6 +88,7 @@ SYMBOLS = {
     "ms_send_json": (C.c_int64, [_P, C.c_char_p]),
     "ms_recv_json": (C.c_int, [_P, C.c_uint32, C.c_int64, C.c_char_p, C.c_size_t]),
     "ms_add_gen_clients": (C.c_int, [_P, _P, C.c_uint32]),
+    "ms_add_kv_clients": (C.c_int, [_P, _P, C.c_uint32]),
     "ms_history_drain": (C.c_int, [_P, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "ms_schedule_ops": (C.c_int, [_P, _P, C.c_size_t]),
     "ms_step": (C.c_int, [_P, C.c_uint64]),

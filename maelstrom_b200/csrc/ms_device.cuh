@@ -240,6 +240,10 @@ struct Params {
   uint4*    rf_heap_sh[8];
   uint64_t* rf_ext_off_sh[8];
   uint32_t* rf_ext_tag_sh[8];
+  // closed-loop lin-kv clients (ms_add_kv_clients): they share gc, gc_hist, gc_n and the gc_*_ns above.
+  // Appended, so that nothing the other kernels read from Params moves
+  uint32_t  kv_value_range, kv_keys_per_group;
+  int64_t   kv_key_period_ns;
 };
 
 constexpr uint32_t kRaftCallbacks = 4096;       // default pending-RPC table slots per node (ms_config.reserved[5]; oracle: same)
@@ -283,10 +287,13 @@ struct GenDev {
   int64_t  deadline_ns;                // when the outstanding request times out (client.clj:96-101)
   int64_t  next_op_ns;                 // stagger: earliest time of the next invocation
   uint32_t node;                       // the server this client talks to
-  uint32_t ops, bcasts;                // ops invoked so far, broadcasts among them
+  uint32_t ops;                        // ops invoked so far
+  union { uint32_t bcasts;             // broadcasts among them
+          uint32_t key_base; };        // lin-kv client: first key of its group's range
   uint32_t phase;                      // 0 mix, 1 quiet period, 2 final read outstanding, 3 done
   uint32_t cur_f, cur_value;           // the op in flight
-  uint32_t ordinal, pad;               // k of client k
+  uint32_t ordinal;                    // k of client k
+  uint32_t reader;                     // lin-kv client: 1 = only reads (gen/reserve)
 };
 enum : uint32_t { GEN_MIX = 0, GEN_QUIET = 1, GEN_FINAL = 2, GEN_DONE = 3 };
 

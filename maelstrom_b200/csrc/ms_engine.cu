@@ -1067,6 +1067,69 @@ int ms_add_gen_clients(ms_sim* s, const ms_gen_config* gc, uint32_t first_name) 
   return (int)first;
 }
 
+// Closed-loop lin-kv clients of the Raft nodes: n endpoints "c<first_name>..", 2g per group, a group per
+// cluster, driven by kv_gen_step inside the Raft family's round kernel (csrc/ms_kernels.cu).
+int ms_add_kv_clients(ms_sim* s, const ms_kv_gen_config* kc, uint32_t first_name) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  if (!kc || kc->n_clients == 0 || kc->interval_ns <= 0 || kc->keys_per_group == 0 || kc->key_period_ns <= 0 ||
+      kc->value_range > 256 || kc->timeout_ns < 0) {
+    set_err("ms_add_kv_clients: bad configuration");
+    return MS_ERR_ARG;
+  }
+  if (s->cfg.workload != MS_W_RAFT) { set_err("ms_add_kv_clients: the lin-kv clients drive the Raft nodes (MS_W_RAFT)"); return MS_ERR_ARG; }
+  if (s->P.gc) { set_err("ms_add_kv_clients: the generator's clients exist already"); return MS_ERR_ARG; }
+  if (s->P.n_shards > 1) { set_err("ms_add_kv_clients: single GPU only"); return MS_ERR_ARG; }
+  Params& P = s->P;
+  const uint32_t gsz = P.rf_group ? P.rf_group : s->cfg.n_nodes;            // servers per cluster
+  const uint32_t n_clusters = s->cfg.n_nodes / gsz;                         // whole clusters
+  if (kc->n_clients % (2u * gsz)) {
+    set_err("ms_add_kv_clients: n_clients must be a multiple of twice the cluster size (" + std::to_string(2u * gsz) + ")");
+    return MS_ERR_ARG;
+  }
+  const uint32_t n_groups = kc->n_clients / (2u * gsz);
+  const uint64_t keys = (uint64_t)((n_groups + n_clusters - 1u) / n_clusters) * kc->keys_per_group;   // per cluster
+  if (keys > std::min<uint64_t>(P.rf_n_keys, 1u << 16)) {
+    set_err("ms_add_kv_clients: the groups of a cluster need " + std::to_string(keys) + " keys, more than ms_config.reserved[2] or 65536");
+    return MS_ERR_ARG;
+  }
+  if ((uint64_t)P.n_ep + kc->n_clients > s->cfg.max_endpoints) { set_err("max_endpoints exhausted"); return MS_ERR_CAPACITY; }
+  for (uint32_t k = 0; k < kc->n_clients; k++)
+    if (s->by_name.count("c" + std::to_string(first_name + k))) { set_err("endpoint already exists: c" + std::to_string(first_name + k)); return MS_ERR_ARG; }
+  int rc;
+  const uint32_t hist_cap = pow2_at_least(std::max<uint32_t>(1u << 16, 64u * kc->n_clients));
+  if ((rc = s->dalloc(&P.gc, s->cfg.max_endpoints)) || (rc = s->dalloc(&P.gc_hist, (size_t)hist_cap * 2))) return rc;
+  P.gc_hist_mask = hist_cap - 1u;
+  P.gc_n = kc->n_clients;
+  P.gc_interval_ns = kc->interval_ns;
+  P.gc_timeout_ns = kc->timeout_ns > 0 ? kc->timeout_ns
+                                       : (int64_t)std::max<uint64_t>(10ull * s->cfg.latency_mean_ms, 1000ull) * kTickNs;   // lin_kv.clj:54
+  P.gc_limit_ns = kc->time_limit_ns;
+  P.kv_value_range = kc->value_range ? kc->value_range : 5u;                // (rand-int 5)
+  P.kv_keys_per_group = kc->keys_per_group;
+  P.kv_key_period_ns = kc->key_period_ns;
+  const uint32_t first = P.n_ep;
+  std::vector<GenDev> init(kc->n_clients);
+  memset(init.data(), 0, init.size() * sizeof(GenDev));
+  for (uint32_t k = 0; k < kc->n_clients; k++) {
+    const std::string id = "c" + std::to_string(first_name + k);
+    const uint32_t idx = first + k, group = k / (2u * gsz);
+    s->kinds[idx] = MS_KIND_GEN_CLIENT;
+    s->names.push_back(id);
+    s->mailbox.emplace_back();
+    s->by_name[id] = idx;
+    init[k].node = (group % n_clusters) * gsz + k % gsz;
+    init[k].key_base = (group / n_clusters) * kc->keys_per_group;
+    init[k].reader = k % (2u * gsz) < gsz;
+    init[k].ordinal = k;
+  }
+  P.n_ep = first + kc->n_clients;
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(P.kind + first, s->kinds.data() + first, kc->n_clients, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(P.gc + first, init.data(), init.size() * sizeof(GenDev), cudaMemcpyHostToDevice));
+  return (int)first;
+}
+
 int ms_history_drain(ms_sim* s, ms_hist* out, size_t cap, size_t* n_out) {
   std::lock_guard<std::mutex> g(s->mu);
   cudaSetDevice(s->device);

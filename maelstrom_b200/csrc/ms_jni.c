@@ -91,6 +91,11 @@ jint FN(addGenClients)(JNIEnv* env, jclass c, jlong h, jobject cfg, jint firstNa
   (void)c;
   return ms_add_gen_clients(H(h), (const ms_gen_config*)BUF(cfg), (uint32_t)firstName);
 }
+/* the lin-kv clients of the Raft nodes: cfg = direct buffer holding an ms_kv_gen_config */
+jint FN(addKvClients)(JNIEnv* env, jclass c, jlong h, jobject cfg, jint firstName) {
+  (void)c;
+  return ms_add_kv_clients(H(h), (const ms_kv_gen_config*)BUF(cfg), (uint32_t)firstName);
+}
 jlong FN(historyDrain)(JNIEnv* env, jclass c, jlong h, jobject out, jlong cap) {
   (void)c;
   size_t n = 0;

@@ -530,6 +530,69 @@ __device__ bool gen_step(const Params& p, DevState* st, uint32_t e, int64_t now,
   return send;
 }
 
+// The lin-kv client of the Raft nodes (ms_add_kv_clients, DESIGN.md 2.12): the client side of gen_step with the
+// generator of workload/lin_kv.clj:78-85; the oracle's twin is tests/native/kv_oracle.cpp.  gen_timer_due holds for it
+// as it is: a client is due for its deadline, its next op or the time limit, and GEN_DONE is never due.
+__device__ bool kv_gen_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const uint4* myring,
+                            uint32_t head, uint32_t my_mask, uint32_t n, const uint16_t* ord, const uint32_t* vals, Rec& out) {
+  GenDev g = p.gc[e];
+  for (uint32_t pos = 0; pos < n; pos++) {
+    const uint32_t i = ord[pos];
+    if (!(vals[i] & (1u << 30))) continue;                                 // V_RECV: cut by a partition
+    const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
+    const uint4 vb = rp[1], vc = rp[2];
+    const uint32_t type = vc.x & 0xFFFFu, flags = vc.x >> 16;
+    // only in_reply_to is matched: a proxied request is answered by the leader (raft.py:558-561)
+    if (!g.waiting_for || !(flags & MS_F_REPLY) || vb.w != g.waiting_for) continue;   // client.clj:106-107
+    uint32_t outcome = MS_H_OK, err = 0, value = g.cur_value;
+    if (type == MS_T_ERROR) {                                              // lin_kv.clj:52: #{:read} is idempotent
+      err = vc.y;
+      const bool definite = err != 0 && err != 13;
+      outcome = (definite || g.cur_f == MS_HF_KV_READ) ? MS_H_FAIL : MS_H_INFO;
+    } else if (g.cur_f == MS_HF_KV_READ) {
+      value |= (vc.z & 0xFFu) << 16;                                       // read_ok: the value is in p1
+    }
+    gen_hist(p, st, now, round, e, g, g.ops, outcome, g.cur_f, err, value);
+    g.waiting_for = 0;
+  }
+  if (g.waiting_for && now >= g.deadline_ns) {
+    gen_hist(p, st, now, round, e, g, g.ops, g.cur_f == MS_HF_KV_READ ? MS_H_FAIL : MS_H_INFO, g.cur_f, MS_H_TIMEOUT, g.cur_value);
+    g.waiting_for = 0;
+  }
+  bool send = false;
+  if (!g.waiting_for && g.phase == GEN_MIX) {
+    if (now >= p.gc_limit_ns) {
+      g.phase = GEN_DONE;
+    } else if (now >= g.next_op_ns) {
+      uint32_t x[4];
+      philox4x32_10(g.ops, e, 0xC11E47u, 0u, p.seed_lo, p.seed_hi, x);     // the client's own stream: op k
+      const uint32_t key = g.key_base + (uint32_t)((uint64_t)(now / p.kv_key_period_ns) % p.kv_keys_per_group);
+      const uint32_t a = (uint32_t)(((uint64_t)x[2] * p.kv_value_range) >> 32);
+      const uint32_t b = (uint32_t)(((uint64_t)x[3] * p.kv_value_range) >> 32);
+      uint32_t f = MS_HF_KV_READ, wtype = MS_T_READ;
+      out.p1 = 0;
+      if (!g.reader) {
+        if ((((uint64_t)x[0] * 3u) >> 32) == 0) { f = MS_HF_KV_WRITE; wtype = MS_T_WRITE; out.p1 = a; }
+        else { f = MS_HF_KV_CAS; wtype = MS_T_CAS; out.p1 = (uint64_t)a | ((uint64_t)b << 32); }
+      }
+      g.next_op_ns = now + (int64_t)(((unsigned __int128)x[1] * (unsigned __int128)(2 * (uint64_t)p.gc_interval_ns)) >> 32);
+      g.ops++;
+      g.cur_f = f;
+      g.cur_value = key | (f == MS_HF_KV_READ ? 0u : a << 16) | (f == MS_HF_KV_CAS ? b << 24 : 0u);
+      g.waiting_for = ++g.next_msg_id;                                     // client.clj:61-64
+      g.deadline_ns = now + p.gc_timeout_ns;
+      gen_hist(p, st, now, round, e, g, g.ops, MS_H_INVOKE, f, 0, g.cur_value);
+      out.round = 0; out.ticket = 0; out.idx = 0;
+      out.src = e; out.dest = g.node; out.msg_id = g.waiting_for; out.in_reply_to = 0;
+      out.tf = wtype | ((uint32_t)MS_F_MSG_ID << 16);
+      out.p0 = key;
+      send = true;
+    }
+  }
+  p.gc[e] = g;
+  return send;
+}
+
 #include "ms_tree.h"
 #include "ms_raft.cuh"
 
@@ -1872,10 +1935,14 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       // ---- closed-loop client: replies in id order, timeout, at most one new request (gen_step)
       if (tid == 0) {
         Rec q;
-        const bool send = gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
+        bool send;
+        // the Raft family's clients are the lin-kv ones (ms_add_kv_clients); their requests carry a p1
+        if constexpr (RF) send = kv_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
+        else send = gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
         if (send) {
           s_gen[0] = make_uint4(q.src, q.dest, q.msg_id, q.in_reply_to);
-          s_gen[1] = make_uint4(q.tf, q.p0, 0u, 0u);
+          if constexpr (RF) s_gen[1] = make_uint4(q.tf, q.p0, (uint32_t)q.p1, (uint32_t)(q.p1 >> 32));
+          else s_gen[1] = make_uint4(q.tf, q.p0, 0u, 0u);
         }
         s_misc[2] = send ? 1u : 0u;
       }
@@ -2151,7 +2218,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         }
       }
       if constexpr (RF) {
-        if (valid && j < n_timer) {          // staged by the node's sequential step, in program order
+        if (is_server && valid && j < n_timer) {   // staged by the node's sequential step, in program order (a lin-kv client's request is not staged)
           timer_emission = true;
           const uint4* at = p.rf_stage + ((size_t)e * p.rf_stage_cap + j) * 3;
           const uint4 a = at[0], b = at[1];
@@ -2164,6 +2231,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         const uint4 a = s_gen[0], b = s_gen[1];
         r.src = a.x; r.dest = a.y; r.msg_id = a.z; r.in_reply_to = a.w;
         r.tf = b.x; r.p0 = b.y; r.p1 = 0;
+        if constexpr (RF) r.p1 = (uint64_t)b.z | ((uint64_t)b.w << 32);
       }
       if (valid && !timer_emission) {
         const uint32_t jm = j - n_timer;       // index among the emissions caused by messages

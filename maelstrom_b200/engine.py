@@ -158,6 +158,18 @@ class Sim:
         gc = _lib.GenConfig(n_clients, read_permille, interval_ns, timeout_ns, time_limit_ns, quiet_ns)
         return self._chk(self.L.ms_add_gen_clients(self.h, C.byref(gc), first_name))
 
+    def add_kv_clients(self, n_clients, interval_ns, time_limit_ns, key_period_ns, keys_per_group=1, value_range=0,
+                       timeout_ns=0, first_name=0):
+        """ms_add_kv_clients: closed-loop lin-kv clients of the Raft nodes on the device (groups of 2g per key,
+        half of them readers); returns the first endpoint index.  history() returns their records,
+        kv_history(records, *sim.kv_groups) sorts them into one history per register"""
+        kc = _lib.KvGenConfig(n_clients, value_range, keys_per_group, interval_ns, timeout_ns, time_limit_ns,
+                              key_period_ns)
+        first = self._chk(self.L.ms_add_kv_clients(self.h, C.byref(kc), first_name))
+        g = int(self.cfg.reserved[4])
+        self.kv_groups = (first, 2 * (g if 0 < g < self.n_nodes else self.n_nodes))   # first client, clients per group
+        return first
+
     def history(self, cap=1 << 20):
         """ms_history_drain: the history records since the last call, in (time, round, client) order"""
         parts = []
@@ -391,6 +403,34 @@ class Sim:
         d["voted_for"] -= 1
         d["leader"] -= 1
         return d
+
+
+HIST_TYPES = ("invoke", "ok", "fail", "info")              # MS_H_*
+HF_KV_READ, HF_KV_WRITE, HF_KV_CAS = 2, 3, 4              # MS_HF_KV_*
+
+
+def kv_history(records, first_client, group_clients):
+    """The lin-kv clients' records (Sim.history() after add_kv_clients; first_client, group_clients =
+    Sim.kv_groups) as the histories a register checker consumes: {(group, key): [op, ...]} in history order,
+    one per register -- a group works on one cluster, so equal keys of different groups are different
+    registers.  Each op is {"process", "type", "f", "value", "time", "error"} in Jepsen's shape for independent
+    keys: value (k, v) for a read (v None unless it is an :ok) and a write, (k, (from, to)) for a cas;
+    process = the client's endpoint index."""
+    out = {}
+    for r in records:
+        f, v = int(r["f"]), int(r["value"])
+        k, a, b = v & 0xFFFF, (v >> 16) & 0xFF, v >> 24
+        if f == HF_KV_READ:
+            name, val = "read", (k, a if r["type"] == 1 else None)
+        elif f == HF_KV_WRITE:
+            name, val = "write", (k, a)
+        elif f == HF_KV_CAS:
+            name, val = "cas", (k, (a, b))
+        else:
+            raise ValueError("not a lin-kv history record: f = %d" % f)
+        out.setdefault(((int(r["client"]) - first_client) // group_clients, k), []).append({"process": int(r["client"]), "type": HIST_TYPES[int(r["type"])], "f": name,
+                                      "value": val, "time": int(r["time_ns"]), "error": int(r["error"]) or None})
+    return out
 
 
 def topology(name, n, node):

@@ -134,8 +134,75 @@ def bench_raft(mb, n, virtual_ms, writes_per_tick):
     return out
 
 
+def card():
+    """name and power limit of the GPU, read next to the measurement they belong to"""
+    import subprocess
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return out[0] if out else "unknown"
+    except (OSError, subprocess.SubprocessError):
+        return "unknown"
+
+
+def bench_kv_clients(mb, n, group, steps, step_ms=200, interval_ms=1000):
+    """BASELINE config 4's shape closed loop: clusters of `group` Raft nodes, 2 lin-kv clients per node on the
+    device (ms_add_kv_clients), the partition nemesis of bench.py --config raft64k (random halves at every even
+    virtual second, healed at every odd one; the default 12 steps after the warm-up step see one such cycle).  The history is drained after every step, as a checker's feed
+    would; device time is the engine's CUDA-event timer around each step's rounds."""
+    from maelstrom_b200.engine import KIND_SIM_CLIENT, OP_DTYPE, TYPES, F_MSG_ID
+    n_clients = (2 * n) // (2 * group) * (2 * group)
+    sim = mb.Sim(n, workload="lin-kv", latency_dist="constant", latency_mean_ms=0, journal_level=0,
+                 max_endpoints=n + n_clients + 8, ring_cap=256, max_window=128, server_ring_cap=64, server_max_window=32,
+                 raft_group=group, rpc_table=64, n_keys=16, raft_log_cap=2048)
+    c = sim.add_endpoint("c%d" % n_clients, KIND_SIM_CLIENT)
+    rows = ops_array(n, OP_DTYPE)
+    rows["src"], rows["dest"] = c, np.arange(n)
+    rows["time_ns"] = np.arange(n) // 128 * 1_000_000   # the sink's inbox takes 128 init_ok per round
+    ramp_ms = 4600 + -(-(n // 128) // step_ms) * step_ms
+    rows["body"]["type"], rows["body"]["flags"], rows["body"]["msg_id"] = TYPES["init"], F_MSG_ID, np.arange(n) + 1
+    sim.schedule(rows)
+    sim.run(ramp_ms * 1_000_000)                       # the first elections happen 2-4 s after init (raft.py:249-251)
+    sim.add_kv_clients(n_clients, interval_ns=interval_ms * 1_000_000, time_limit_ns=1 << 62,
+                       key_period_ns=1_000_000_000, keys_per_group=16)
+    rng = np.random.default_rng(0x4D41454C)
+    tally = np.zeros(4, dtype=np.int64)                # invoke / ok / fail / info
+    dev_ms = wall = 0.0
+    m0 = r0 = 0
+    for k in range(steps + 1):                         # step 0 is the warm-up: not timed, not counted
+        now_ms = ramp_ms + k * step_ms
+        if now_ms % 1000 == 0:
+            if (now_ms // 1000) % 2 == 0:
+                sim.partition(rng.integers(0, 2, size=n).astype(np.uint32))
+            else:
+                sim.heal()
+        t0 = time.time()
+        sim.timer_begin()
+        sim.run((now_ms + step_ms) * 1_000_000)
+        ms = sim.timer_end()                           # ends in a synchronise on the event
+        h = sim.history()
+        dt = time.time() - t0
+        if k == 0:
+            m0, r0 = sim.stats()["all"]["msg-count"], sim.counters()["recvs"]
+            continue
+        dev_ms += ms
+        wall += dt
+        tally += np.bincount(h["type"], minlength=4)[:4]
+    msgs = sim.stats()["all"]["msg-count"] - m0
+    recvs = sim.counters()["recvs"] - r0
+    done = int(tally[1:].sum())
+    return dict(workload="lin-kv (Raft), closed-loop clients on the device", nodes=n, cluster_size=group,
+                clients=n_clients, virtual_ms=steps * step_ms, client_interval_ms=interval_ms, latency="constant 0 ms",
+                nemesis="random halves for 1 s, healed for 1 s", device_ms=dev_ms, wall_s=wall, rounds=sim.counters()["rounds"],
+                ops_invoked=int(tally[0]), ops_completed=done, ok=int(tally[1]), fail=int(tally[2]), info=int(tally[3]),
+                ops_per_s_wall=done / wall if wall > 0 else None,
+                msgs_per_s=recvs / (dev_ms / 1e3) if dev_ms > 0 else None,
+                msgs_per_op=msgs / int(tally[0]) if tally[0] else None, card=card())
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--only", default="", help="run one case: g-set, services, txn, raft or kv-clients")
     ap.add_argument("--emul", action="store_true", help="run on the CPU SIMT emulator (script check only)")
     ap.add_argument("--tiny", action="store_true")
     a = ap.parse_args()
@@ -147,13 +214,16 @@ def main():
         ctx.__enter__()
     try:
         if a.tiny:
-            runs = [lambda: bench_gset(mb, 12, 8, 512, 10, 4), lambda: bench_services(mb, 40, 5),
-                    lambda: bench_txn(mb, 3, 12, 5), lambda: bench_raft(mb, 3, 4260, 2)]
+            runs = {"g-set": lambda: bench_gset(mb, 12, 8, 512, 10, 4), "services": lambda: bench_services(mb, 40, 5),
+                    "txn": lambda: bench_txn(mb, 3, 12, 5), "raft": lambda: bench_raft(mb, 3, 4260, 2),
+                    "kv-clients": lambda: bench_kv_clients(mb, 11, 5, 3)}
         else:
-            runs = [lambda: bench_gset(mb, 1024, 100, 1 << 14, 200, 64), lambda: bench_services(mb, 1 << 14, 20),
-                    lambda: bench_txn(mb, 256, 1 << 11, 20), lambda: bench_raft(mb, 5, 10_000, 4)]
-        for r in runs:
-            print(json.dumps(r(), sort_keys=True), flush=True)
+            runs = {"g-set": lambda: bench_gset(mb, 1024, 100, 1 << 14, 200, 64), "services": lambda: bench_services(mb, 1 << 14, 20),
+                    "txn": lambda: bench_txn(mb, 256, 1 << 11, 20), "raft": lambda: bench_raft(mb, 5, 10_000, 4),
+                    "kv-clients": lambda: bench_kv_clients(mb, 65536, 5, 12)}
+        for name, r in runs.items():
+            if not a.only or a.only == name:
+                print(json.dumps(r(), sort_keys=True), flush=True)
     finally:
         if ctx:
             ctx.__exit__(None, None, None)
