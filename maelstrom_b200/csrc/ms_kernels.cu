@@ -1563,7 +1563,9 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
   cx.need_rng = need_rng;
   cx.const_lat = const_lat;
   cx.c_send_cl = cx.c_send_sv = cx.c_lost = cx.c_zero = 0;
-  uint32_t c_recv_cl = 0, c_recv_sv = 0, c_part = 0, c_replies = 0;
+  // per-thread counters of what the scan totals do not give: receives from clients (the servers' share is
+  // n_recv minus these, partition drops are n - n_recv: both stored by one thread in PD), replies to clients
+  uint32_t c_recv_cl = 0, c_replies = 0;
   uint32_t n_ev_local = 0, n_em_local = 0;
 
   if (ticket < p.n_inj_tickets) {
@@ -2111,6 +2113,8 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     if (timing && tid == 0 && n > 1) atomicAdd((unsigned long long*)&p.phase_cycles[cls * 16 + 13], (unsigned long long)R);
     if (tid == 32 % nt) {
       journal_claim(p, st, n_ev_local, ticket, s_chunk);
+      s_cnt[3] = n_recv;                      // receives from servers, less the epilogue's client-sourced ones
+      s_cnt[6] = n - n_recv;                  // cut by a partition at dequeue
       if (mailed && n_recv) s_misc[0] = atomicAdd(&st->mail_count, n_recv);
     }
     if (agg && tid < (int)deg) {   // deg <= MAXNB <= 32 <= blockDim
@@ -2135,6 +2139,10 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         const uint32_t o = owner_of(nb, p.n_servers, p.n_shards);
         const uint32_t ci = compact ? p.cq + nb : nb;      // the compact ring's counters, or the 48-B ring's
         base = atomicAdd(&p.tail_sh[o][ci], total);
+        if (compact) {                        // PE2's fast path writes exactly these: server sends, zero latency
+          atomicAdd(&s_cnt[1], total);
+          atomicAdd(&s_cnt[5], total);
+        }
         if ((uint32_t)(base + total - p.head_sh[o][ci]) > ring_cap_of(p, nb)) latch_error(st, E_RING_OVERFLOW, nb);
       }
       s_nbbase[tid] = base;
@@ -2157,7 +2165,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     for (uint32_t pos = tid; pos < n; pos += nt) {
       const uint32_t i = ord[pos];
       const uint32_t val = vals[i];
-      if (!(val & V_RECV)) { c_part++; continue; }
+      if (!(val & V_RECV)) continue;
       const uint32_t k = (uint32_t)(aux[pos] >> 32) & 0xFFFFu;
       const uint32_t mt = meta[i];
       const uint32_t sslot = mt & M_SRCSLOT;
@@ -2166,7 +2174,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         const uint64_t id = (use_blocks ? s_bbase[blk[pos]] : dense_base(p, st, m.round, m.ticket)) + m.idx;
         journal_raw(p, cx.chunk + k, id, true, m);
         const bool cl = cl_ep || (m.src >= p.n_servers && kind_is_client(p.kind[m.src]));
-        if (cl) c_recv_cl++; else c_recv_sv++;
+        if (cl) c_recv_cl++;
         if (kind == MS_KIND_SIM_CLIENT && ((m.tf >> 16) & MS_F_REPLY)) c_replies++;
         if (mailed) {
           const uint32_t mpos = s_misc[0] + k;
@@ -2186,7 +2194,6 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         if (p.jlevel)
           st_v4(p.jraw + ((cx.chunk + k) & p.jmask),
                 make_uint4((uint32_t)vrec, (uint32_t)(vrec >> 32), s_nbr[sslot - 1], e));
-        c_recv_sv++;
       }
     }
     // PE2: emissions in id order, one emission per thread: emission j belongs to the last
@@ -2304,9 +2311,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
         // server -> neighbor gossip into compact ring space this CTA already claimed: what emit_one does for it,
         // without the general case's lookups (both ends are live servers, zero constant latency, no loss: agg_ok)
         r.round = round; r.ticket = ticket; r.idx = j;                         // order key == id order (net.clj:197)
-        journal_raw(p, cx.chunk + n_recv + j, j, false, r);                    // net.clj:208
-        cx.c_send_sv++;
-        cx.c_zero++;
+        journal_raw(p, cx.chunk + n_recv + j, j, false, r);                    // net.clj:208 (counted in PD)
         uint4* ring_o = p.ring_sh[owner_of(r.dest, p.n_servers, p.n_shards)];
         st_v4(cring_slot(p, ring_o, r.dest, direct), make_uint4(j, ticket, (uint32_t)round, r.p0));
       }
@@ -2335,12 +2340,18 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
   PHASE_MARK(6);
   // ------------------------------------------------------------ ticket epilogue
   {
-    uint32_t cnt[8] = {cx.c_send_cl, cx.c_send_sv, c_recv_cl, c_recv_sv, cx.c_lost, cx.c_zero, c_part, c_replies};
+    // s_cnt: 0 send cl, 1 send sv, 2 recv cl, 3 recv sv, 4 lost, 5 zero latency, 6 partition drops, 7 client replies.
+    // A warp of a gossip window has nothing to add: its sends and receives were counted from the totals in PD.
+    uint32_t cnt[6] = {cx.c_send_cl, cx.c_send_sv, c_recv_cl, cx.c_lost, cx.c_zero, c_replies};
+    constexpr int at[6] = {0, 1, 2, 4, 5, 7};
+    if (__any_sync(FULL, (cnt[0] | cnt[1] | cnt[2] | cnt[3] | cnt[4] | cnt[5]) != 0)) {
 #pragma unroll
-    for (int q = 0; q < 8; q++) {
+      for (int q = 0; q < 6; q++) {
 #pragma unroll
-      for (int d = 16; d > 0; d >>= 1) cnt[q] += __shfl_xor_sync(FULL, cnt[q], d);
-      if (lane == 0 && cnt[q]) atomicAdd(&s_cnt[q], cnt[q]);
+        for (int d = 16; d > 0; d >>= 1) cnt[q] += __shfl_xor_sync(FULL, cnt[q], d);
+        if (lane == 0 && cnt[q]) atomicAdd(&s_cnt[at[q]], cnt[q]);
+      }
+      if (lane == 0 && cnt[2]) atomicAdd(&s_cnt[3], 0u - cnt[2]);
     }
   }
   __syncthreads();
