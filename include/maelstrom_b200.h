@@ -301,6 +301,19 @@ int      ms_step(ms_sim* sim, uint64_t n_rounds);       /* exactly n rounds */
 int      ms_run(ms_sim* sim, int64_t until_virtual_ns); /* rounds while now < until */
 int64_t  ms_now(ms_sim* sim);
 uint64_t ms_round(ms_sim* sim);
+/* Idle-time jump, off by default; may be switched between any two calls.  On, ms_run, ms_run_streamed and
+ * the waiting loop of ms_recv / ms_recv_json move virtual time, after a round that advanced it, straight to the
+ * first tick at which some endpoint would act (mail in a ring, a node or client timer, a scheduled op, a
+ * timing-wheel slot coming up), never past the first tick at or after the call's stop time.  The round counter
+ * jumps with time: a jump of k ticks adds k to ms_round, as the k empty rounds it replaces would.  So every
+ * output is byte-identical to the same calls made without the mode: the journal (drained, streamed in every
+ * format, Fressian file), ms_history_drain, ms_stats, ms_node_set, ms_raft_state, ms_client_replies,
+ * ms_undeliverable, ms_now and ms_round after every call.  What differs: ms_counters' rounds and launches count
+ * what the GPU executed (ms_round - origin - rounds = rounds jumped; two launches more per executed round), and
+ * wall time.  ms_step(n) still runs exactly n rounds and never jumps.  With the journal kept, a jump stops where
+ * the round history needs a drain, as the rounds it replaces would have.  MS_ERR_ARG on a sharded simulation
+ * (the jump would need the minimum over all shards) and with CUDA-graph replay (ms_config.reserved[1] = 1). */
+int      ms_set_idle_jump(ms_sim* sim, int enable);
 
 /* ------------------------------------------------------------------ faults: jepsen-net (net.clj:105-122) */
 int ms_net_drop(ms_sim* sim, uint32_t src, uint32_t dest);   /* partitions[dest] += src */

@@ -32,6 +32,7 @@ public final class Native {
   public static native int run(long h, long untilNs);
   public static native long now(long h);
   public static native long round(long h);
+  public static native int setIdleJump(long h, int enable);
   public static native int netDrop(long h, int src, int dest);
   public static native int netHeal(long h);
   public static native int netSlow(long h);

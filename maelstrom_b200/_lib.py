@@ -95,6 +95,7 @@ SYMBOLS = {
     "ms_run": (C.c_int, [_P, C.c_int64]),
     "ms_now": (C.c_int64, [_P]),
     "ms_round": (C.c_uint64, [_P]),
+    "ms_set_idle_jump": (C.c_int, [_P, C.c_int]),
     "ms_net_drop": (C.c_int, [_P, C.c_uint32, C.c_uint32]),
     "ms_net_heal": (C.c_int, [_P]),
     "ms_net_slow": (C.c_int, [_P]),

@@ -75,6 +75,9 @@ struct DevState {
   uint32_t cls_count[2][4];   // tickets at the front of the class list (the longer windows)
   uint32_t cls_small[2][4];   // tickets at the back of the class list
   uint32_t cls_cursor[2][4];
+  // idle-time jump (ms_set_idle_jump): ~(earliest instant at which an endpoint acts), folded in by k_wake with
+  // atomicMax (a minimum of the instant), 0 = none; consumed and cleared by k_jump.  Appended: nothing moves
+  uint64_t idle_wake;
 };
 
 // One row per round, kept in a ring of `hist` rounds: what is needed to turn an

@@ -32,6 +32,7 @@ void msk_launch_round(const msd::Params* p, int n_classes, const uint32_t* caps,
                       cudaEvent_t after_round, int phases, const cudaStream_t* aux, const cudaEvent_t* aux_ev);
 void msk_set_bit(uint32_t* words, size_t word, uint32_t bit, cudaStream_t s);
 void msk_barrier(const msd::Params* p, cudaStream_t s);
+void msk_launch_idle_jump(const msd::Params* p, cudaStream_t s);
 void msk_journal_expand(const msd::Params* p, uint64_t r0, uint32_t n_rounds, uint64_t first, uint64_t count,
                         void* out_ev, void* out_body, int n_sms, cudaStream_t s);
 size_t msk_stream_plan_bytes();
@@ -149,6 +150,7 @@ struct ms_sim {
   // a fixed batch wastes launches on rounds past the stop time and a blocking read-back per batch
   uint64_t run_hint = 0;
   bool mail_seen = false;          // host-visible deliveries happened: keep the batches short (mail_cap)
+  bool idle_jump = false;          // ms_set_idle_jump: ms_run / ms_run_streamed / ms_recv jump over idle ticks
 
   std::vector<uint8_t> kinds;
   std::vector<std::string> names;
@@ -282,9 +284,10 @@ struct ms_sim {
     return MS_OK;
   }
 
-  void launch_rounds(uint64_t n) {
+  // jump: every round is preceded by the idle-time jump (k_wake | k_jump, ms_set_idle_jump)
+  void launch_rounds(uint64_t n, bool jump = false) {
     // batches of rounds are replayed from a CUDA graph: removes the per-launch host cost
-    if (use_graph && !profiling && !barrier && n >= 8) {
+    if (use_graph && !jump && !profiling && !barrier && n >= 8) {
       if (graph_exec && (graph_rounds != n || memcmp(&graph_P, &P, sizeof(Params)) != 0)) {
         cudaGraphExecDestroy(graph_exec);
         graph_exec = nullptr;
@@ -313,10 +316,10 @@ struct ms_sim {
         return;
       }
     }
-    launch_rounds_direct(n);
+    launch_rounds_direct(n, jump);
   }
 
-  void launch_rounds_direct(uint64_t n) {
+  void launch_rounds_direct(uint64_t n, bool jump = false) {
     // sharded, no timing wheel, the engine's own barrier, few enough endpoints for one CTA: one glue launch between rounds
     const bool glue = P.n_shards > 1 && !use_calendar && !barrier && !P.cm_blk && P.n_ep <= 32768 && !getenv("MS_NO_GLUE");
     for (uint64_t i = 0; i < n; i++) {
@@ -335,6 +338,10 @@ struct ms_sim {
       int grids[4];
       for (int c = 0; c < n_classes; c++) grids[c] = std::max(1, std::min(class_grid[c], T));
       if (P.n_shards <= 1) {
+        if (jump) {
+          msk_launch_idle_jump(&P, stream);
+          if (!capturing()) launches += 2;
+        }
         msk_launch_round(&P, n_classes, class_cap, class_threads, grids, use_calendar ? 1 : 0, stream, a, b, 15, aux_streams, aux_events);
         if (!capturing()) launches += (use_calendar ? 2 : 1) + n_classes + (P.split_commit ? (P.cm_blk ? 3 : 1) : 0);
       } else if (glue) {
@@ -1219,7 +1226,7 @@ static bool journal_blocked(const ms_sim* s) {
   return s->hs.round - s->hs.drain_round + 2 >= s->P.hist;
 }
 
-static int step_locked(ms_sim* s, uint64_t n_rounds, int64_t stop) {
+static int step_locked(ms_sim* s, uint64_t n_rounds, int64_t stop, bool jump = false) {
   cudaSetDevice(s->device);
   int rc;
   if (s->P.n_shards > 1) {
@@ -1228,7 +1235,7 @@ static int step_locked(ms_sim* s, uint64_t n_rounds, int64_t stop) {
   }
   if ((rc = s->stage_injections())) return rc;
   if ((rc = s->set_stop(stop))) return rc;
-  s->launch_rounds(n_rounds);
+  s->launch_rounds(n_rounds, jump);
   {
     const cudaError_t le = cudaGetLastError();      // a launch that was refused never shows up in the stream
     if (le != cudaSuccess) { set_err(std::string("kernel launch: ") + cudaGetErrorString(le)); return MS_ERR_CUDA; }
@@ -1307,7 +1314,7 @@ int ms_run(ms_sim* s, int64_t until) {
     const uint64_t r0 = s->hs.rounds_run;
     static const bool dbg_stall = getenv("MS_DEBUG_STALL") != nullptr;   // diagnostic: one round per batch, state on stderr
     if (dbg_stall) batch = 1;
-    const int rc = step_locked(s, batch, until);
+    const int rc = step_locked(s, batch, until, s->idle_jump);
     if (rc) return rc;
     if (dbg_stall && (s->hs.rounds_run == r0 || s->hs.round < 4))
       fprintf(stderr, "MS_DEBUG_STALL advanced=%d%s cursors %u %u %u %u\n", (int)(s->hs.rounds_run - r0), stall_report(s).c_str(),
@@ -1345,8 +1352,10 @@ static int recv_locked(ms_sim* s, uint32_t e, int64_t timeout, ms_msg* out) {
     if (s->hs.now >= give_up) return 0;
     if (journal_blocked(s)) { set_err("journal ring half full: drain it (ms_journal_drain)"); return MS_ERR_CAPACITY; }
     const uint64_t r0 = s->hs.rounds_run;
-    const int rc = step_locked(s, 1, INT64_MAX);
-    if (!rc && s->hs.rounds_run == r0) { set_err("simulation made no progress (device refuses to run rounds)"); return MS_ERR_SIM; }
+    // with the idle-time jump the wait ends at give_up: a jump lands on the first tick at or after it, where the
+    // ticking loop stops too, and runs no round there
+    const int rc = step_locked(s, 1, s->idle_jump ? give_up : INT64_MAX, s->idle_jump);
+    if (!rc && s->hs.rounds_run == r0 && !(s->idle_jump && s->hs.now >= give_up)) { set_err("simulation made no progress (device refuses to run rounds)"); return MS_ERR_SIM; }
     if (rc) return rc;
   }
 }
@@ -1692,7 +1701,7 @@ int ms_run_streamed(ms_sim* s, int64_t until, int format, size_t buf_events, ms_
   int result = MS_OK;
   for (uint64_t i = 0;; i++) {
     const int b = (int)(i & 1), hb = (int)(i & 3);
-    if (launching) s->launch_rounds(batch_rounds);
+    if (launching) s->launch_rounds(batch_rounds, s->idle_jump);
     // what batch i may pack is fixed here, in stream order: the journal stream runs alongside batch i+1's rounds
     msk_stream_mark(&s->P, s->jplan, s->stream, (uint32_t)b);
     CK(cudaEventRecord(s->j_rounds_done[b], s->stream));
@@ -2013,6 +2022,14 @@ int ms_set_origin(ms_sim* s, uint64_t round, uint64_t msg_id, uint64_t event_id,
   CK(cudaMemcpy(P.tail, ctr.data(), n_ctr * 4, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(P.limit, ctr.data(), n_ctr * 4, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(P.head, ctr.data(), n_ctr * 4, cudaMemcpyHostToDevice));
+  return MS_OK;
+}
+
+int ms_set_idle_jump(ms_sim* s, int enable) {
+  std::lock_guard<std::mutex> g(s->mu);
+  if (enable && s->P.n_shards > 1) { set_err("ms_set_idle_jump: a sharded simulation ticks (the jump would need the minimum over all shards)"); return MS_ERR_ARG; }
+  if (enable && s->cfg.reserved[1] == 1) { set_err("ms_set_idle_jump: not with CUDA-graph replay (ms_config.reserved[1] = 1)"); return MS_ERR_ARG; }
+  s->idle_jump = enable != 0;
   return MS_OK;
 }
 

@@ -111,6 +111,7 @@ jint FN(step)(JNIEnv* env, jclass c, jlong h, jlong nRounds) { (void)env; (void)
 jint FN(run)(JNIEnv* env, jclass c, jlong h, jlong untilNs) { (void)env; (void)c; return ms_run(H(h), untilNs); }
 jlong FN(now)(JNIEnv* env, jclass c, jlong h) { (void)env; (void)c; return ms_now(H(h)); }
 jlong FN(round)(JNIEnv* env, jclass c, jlong h) { (void)env; (void)c; return (jlong)ms_round(H(h)); }
+jint FN(setIdleJump)(JNIEnv* env, jclass c, jlong h, jint enable) { (void)env; (void)c; return ms_set_idle_jump(H(h), (int)enable); }
 
 /* jepsen.net.proto/Net (net.clj:105-122) */
 jint FN(netDrop)(JNIEnv* env, jclass c, jlong h, jint src, jint dest) { (void)env; (void)c; return ms_net_drop(H(h), (uint32_t)src, (uint32_t)dest); }

@@ -470,6 +470,13 @@ __device__ __forceinline__ bool gen_timer_due(const Params& p, const GenDev& g, 
   if (g.phase == GEN_QUIET) return now >= p.gc_limit_ns + p.gc_quiet_ns;
   return g.phase == GEN_FINAL;            // the final read has completed or timed out: -> done
 }
+// The earliest instant at which gen_timer_due holds (k_wake, ms_set_idle_jump).  Keep the two in step.
+__device__ __forceinline__ int64_t gen_wake_ns(const Params& p, const GenDev& g) {
+  if (g.waiting_for) return g.deadline_ns;
+  if (g.phase == GEN_MIX) return min(p.gc_limit_ns, g.next_op_ns);
+  if (g.phase == GEN_QUIET) return p.gc_limit_ns + p.gc_quiet_ns;
+  return g.phase == GEN_FINAL ? INT64_MIN : INT64_MAX;
+}
 
 // One step of client e: its due replies in id order, then the timeout, then at most one invocation.
 // Returns true and fills `out` when the step sends a request.
@@ -748,6 +755,56 @@ __device__ void snapshot_endpoints(const Params& p, DevState* st, uint32_t gid, 
   }
 }
 
+// ------------------------------------------------------------------ idle-time jump (ms_set_idle_jump)
+// A round in which no endpoint has a window, no timer is due, nothing is injected and the timing wheel releases
+// nothing only does bookkeeping: k_snapshot finishes every endpoint ticket on the spot and the commit moves time on
+// by one tick.  Between two rounds k_wake finds the earliest instant at which anything can happen and k_jump moves
+// `now` and `round` there together, doing that bookkeeping for the rounds it skips (DESIGN.md 2.3).  Only launched
+// when the mode is on, on one GPU.  Both decide with the same test, on values neither of them changes first.
+__device__ __forceinline__ bool idle_jump_open(const Params& p, const DevState* st) {
+  return p.n_shards <= 1 && st->time_advanced && st->inj_count == 0 && !round_skipped(p, st);
+}
+
+// Grid-stride pass: every condition under which k_snapshot keeps a ticket alive, k_round injects or k_release
+// moves a record, as the instant from which it holds; one atomicMax of ~min per warp into DevState.idle_wake.
+// An earlier instant than needed is harmless (an empty round is ticked), a later one never happens.
+__global__ void k_wake(Params p) {
+  DevState* st = p.st;
+  if (!idle_jump_open(p, st)) return;
+  const int64_t now = st->now;
+  const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+  int64_t w = INT64_MAX;
+  for (uint32_t e = gid; e < p.n_ep; e += stride) {
+    // snapshot_endpoints: a window to consume (a removed endpoint's too: limit <- tail is still to be done)
+    if (p.tail[e] != p.limit[e] || (p.cq && e < p.n_servers && p.tail[p.cq + e] != p.limit[p.cq + e])) w = now;
+    // snapshot_endpoints' timer_due / gen_due
+    if (e < p.n_servers && p.kind[e] == MS_KIND_SERVER) {
+      if (p.workload == MS_W_GSET && p.gs_init[e]) w = min(w, p.gs_next_fire[e]);
+      if (p.workload == MS_W_RAFT) w = min(w, rf_wake_ns(p.rf_node[e]));
+      if (p.workload == MS_W_TXN_TREE) w = min(w, tt_wake_ns(p.tt_node[e]));
+    }
+    if (p.gc && p.kind[e] == MS_KIND_GEN_CLIENT) w = min(w, gen_wake_ns(p, p.gc[e]));
+  }
+  // k_release: slot s comes up at the ticks == s (mod cal_slots).  Either generation counts: records with laps
+  // left are filed again by k_release, so that release has to run too
+  if (p.cal) {
+    const uint64_t t1 = (uint64_t)(now / kTickNs);
+    for (uint32_t s = gid; s < p.cal_slots; s += stride)
+      if (p.cal_count[s] | p.cal_count[p.cal_slots + s])
+        w = min(w, (int64_t)((t1 + ((s - (uint32_t)t1) & (p.cal_slots - 1u))) * (uint64_t)kTickNs));
+  }
+  // k_round's injector slices: the next scheduled op, due in the first round of its tick ceil(time / tick)
+  if (gid == 0 && st->sched_cursor < p.n_sched) {
+    const int64_t t = p.sched[st->sched_cursor].time_ns;
+    w = min(w, t <= 0 ? (int64_t)0 : ((t + kTickNs - 1) / kTickNs) * kTickNs);
+  }
+  if (w < now) w = now;
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) w = min(w, (int64_t)__shfl_xor_sync(FULL, w, d));
+  if ((threadIdx.x & 31) == 0 && w != INT64_MAX)
+    atomicMax((unsigned long long*)&st->idle_wake, (unsigned long long)~(uint64_t)w);
+}
+
 // ------------------------------------------------------------------ k_release (timing wheel -> rings)
 __global__ void k_release(Params p) {
   DevState* st = p.st;
@@ -954,6 +1011,98 @@ __device__ void commit_scalars(const Params& p, DevState* st, uint64_t total, ui
       nx->ev_total = 0;
       nx->em_total = 0;
       __threadfence();
+  }
+}
+
+// One CTA, after k_wake: when the first tick at or after the wake (never past the first tick at or after stop_ns)
+// lies k > 0 ticks ahead, does what the k empty rounds round .. round + k - 1 would have left behind that anything
+// reads later, and opens round + k at now + k ticks.  With the journal kept, k stays inside the round history's
+// headroom (round_skipped's test still passes for the landing round); the host drains and the next batch goes on.
+__global__ void __launch_bounds__(512) k_jump(Params p) {
+  DevState* st = p.st;
+  const uint32_t tid = threadIdx.x, nt = blockDim.x;
+  const int64_t now = st->now;
+  const uint64_t R = st->round;
+  uint64_t k = 0;
+  if (idle_jump_open(p, st)) {
+    const uint64_t inv = st->idle_wake;
+    int64_t t = min(inv ? (int64_t)~inv : INT64_MAX, st->stop_ns);   // > now: round_skipped is false
+    const int64_t t_max = INT64_MAX - 2 * kTickNs;
+    if (t > t_max) t = t_max;
+    k = t > now ? ((uint64_t)(t - now) + kTickNs - 1) / kTickNs : 0;
+    if (p.jlevel && !p.jdiscard) {
+      const uint64_t used = R - st->drain_round + 3;                  // < hist + 1: round R is not skipped
+      const uint64_t room = p.hist > used ? p.hist - used : 0u;
+      if (k > room) k = room;
+    }
+  }
+  __syncthreads();   // every thread has read the state before thread 0 changes it
+  if (k == 0) {
+    if (tid == 0) st->idle_wake = 0;
+    return;
+  }
+  const uint64_t L = R + k;                                   // the landing round
+  const uint64_t t1 = (uint64_t)(now / kTickNs);              // the tick of round R
+  const uint64_t id_base = st->next_id, ev_base = st->next_event, raw_base = st->jraw_cursor;
+  // RoundMeta rows of the skipped rounds and of the landing round, as commit_scalars opens them.  A skipped row
+  // keeps n_tickets = 0: its per-ticket tables are not written, and journal_chunk never looks at them
+  const uint64_t n_rows = k + 1 < p.hist ? k + 1 : p.hist;
+  for (uint64_t j = tid; j < n_rows; j += nt) {
+    const uint64_t r = L - j;
+    RoundMeta* m = p.rmeta + ((uint32_t)r & p.hist_mask);
+    m->round = r;
+    m->now = now + (int64_t)((r - R) * (uint64_t)kTickNs);
+    m->id_base = id_base;
+    m->ev_base = ev_base;
+    m->raw_base = raw_base;
+    m->n_tickets = 0;
+    m->ev_total = 0;
+    m->em_total = 0;
+  }
+  // Per-ticket entries of the skipped rows: tag 0, which no round has.  Ticking rewrites a row every `hist` rounds,
+  // so a stale entry is exactly hist rounds old and its 15-bit round tag differs from the current one; a row left
+  // alone by jumps for a multiple of 2^15 rounds would carry a tag that looks current to the commit's spin-wait
+  const uint32_t T = p.n_inj_tickets + p.n_ep;
+  const uint64_t n_inv = k < p.hist ? k : p.hist;
+  for (uint64_t j = 1; j <= n_inv; j++) {
+    uint64_t* row = p.rt_cnt + (size_t)((uint32_t)(L - j) & p.hist_mask) * p.t_max;
+    for (uint32_t t = tid; t < T; t += nt) row[t] = 0;
+  }
+  // k_snapshot of every skipped round: head <- limit (limit == tail already, or k_wake would have said now)
+  for (uint32_t e = tid; e < p.n_ep; e += nt) {
+    p.head[e] = p.limit[e];
+    if (p.cq && e < p.n_servers) p.head[p.cq + e] = p.limit[p.cq + e];
+  }
+  // timing wheel: the commits of rounds R .. L - 1 flip the slots of ticks t1 + 1 .. t1 + k, one flip per tick
+  // (every slot they pass is empty in both generations, so only the landing slot's parity matters for what is
+  // released next; all of them are kept as ticking leaves them)
+  if (p.cal) {
+    const uint64_t S = p.cal_slots, n_fl = k < S ? k : S;
+    for (uint64_t j = tid; j < n_fl; j += nt) {
+      const uint64_t tick = t1 + 1 + j;
+      if ((((t1 + k - tick) / S) & 1u) == 0) p.cal_par[(uint32_t)tick & (p.cal_slots - 1u)] ^= 1u;   // an odd number of flips
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    if (p.cal) {
+      // k_snapshot of round R: blocks that lost a publish race go back to the pool (the released slot is empty)
+      for (uint32_t i = 0; i < st->cal_ret_n; i++) p.cal_free[st->cal_free_n++] = p.cal_ret[i];
+      st->cal_ret_n = 0;
+      st->cal_release = ((uint32_t)(t1 + k) & (p.cal_slots - 1u)) + 1u;
+    }
+    // k_snapshot clears the class counters of the next round's parity; the landing round's may be stale
+    for (int c = 0; c < 4; c++)
+      for (int q = 0; q < 2; q++) { st->cls_count[q][c] = 0; st->cls_small[q][c] = 0; st->cls_cursor[q][c] = 0; }
+    // commit_scalars of round L - 1
+    const uint64_t tick = t1 + k - 1;
+    const uint32_t hi_s = (tick + 1 < p.n_tick_off) ? p.tick_off[tick + 1] : p.n_sched;
+    if (hi_s > st->sched_cursor) st->sched_cursor = hi_s;
+    if (p.jdiscard || !p.jlevel) st->drain_round = L;
+    st->now = now + (int64_t)(k * (uint64_t)kTickNs);
+    st->round = L;
+    st->idle_wake = 0;
+    __threadfence();
   }
 }
 
@@ -2761,6 +2910,16 @@ void msk_launch_round(const msd::Params* p, int n_classes, const uint32_t* caps,
 }
 
 void msk_barrier(const msd::Params* p, cudaStream_t s) { MS_LAUNCH(msd::k_barrier, 1, 32, 0, s, *p); }
+
+// Idle-time jump between two rounds (ms_set_idle_jump): k_wake over the endpoints and wheel slots, then k_jump.
+void msk_launch_idle_jump(const msd::Params* p, cudaStream_t s) {
+  const uint32_t n = p->cal && p->cal_slots > p->n_ep ? p->cal_slots : p->n_ep;
+  int g = (int)((n + 255u) / 256u);
+  if (g > 2 * (int)p->n_sms) g = 2 * (int)p->n_sms;
+  if (g < 1) g = 1;
+  MS_LAUNCH(msd::k_wake, g, 256, 0, s, *p);
+  MS_LAUNCH(msd::k_jump, 1, 512, 0, s, *p);
+}
 
 size_t msk_stream_plan_bytes() { return sizeof(msd::StreamPlan); }
 // plan -> pack -> finish: one batch of the journal into (host-mapped) `out`, header into `hdr`

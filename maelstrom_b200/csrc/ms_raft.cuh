@@ -393,6 +393,15 @@ __device__ __forceinline__ bool rf_timer_due(const RaftDev& r, int64_t now) {
   const int64_t elapsed = now - r.last_replication;
   return kMinReplicationNs < elapsed && (r.busy || kHeartbeatNs < elapsed);
 }
+// The earliest instant at which rf_timer_due holds (k_wake, ms_set_idle_jump): its guards with their strict `<`.
+// Keep the two in step.
+__device__ __forceinline__ int64_t rf_wake_ns(const RaftDev& r) {
+  auto after = [](int64_t t, int64_t d) { return t > INT64_MAX - d - 1 ? INT64_MAX : t + d + 1; };
+  int64_t w = after(r.election_deadline, 0);
+  if (r.state != RAFT_LEADER) return w;
+  w = min(w, after(r.step_down_deadline, 0));
+  return min(w, after(r.last_replication, r.busy ? kMinReplicationNs : kHeartbeatNs));
+}
 
 // ------------------------------------------------------------------ txn-list-append, single key
 // demo/clojure/single_key_txn.clj: the whole database is one value under key "root" (key 0) of
@@ -671,6 +680,13 @@ __device__ void tt_handle(RaftCtx& c, const Rec& m) {
 // round the clock runs out still counts.  k_snapshot keeps a node's ticket alive when this would act (tt_timer_due).
 __device__ __forceinline__ bool tt_timer_due(const TreeDev& t, int64_t now) {
   return (t.phase != 0 && t.deadline != 0 && now >= t.deadline) || (t.init_phase != 0 && now >= t.init_deadline);
+}
+// The earliest instant at which tt_timer_due holds (k_wake, ms_set_idle_jump).  Keep the two in step.
+__device__ __forceinline__ int64_t tt_wake_ns(const TreeDev& t) {
+  int64_t w = INT64_MAX;
+  if (t.phase != 0 && t.deadline != 0) w = t.deadline;
+  if (t.init_phase != 0) w = min(w, t.init_deadline);
+  return w;
 }
 __device__ void tt_actions(RaftCtx& c) {
   TreeDev* t = c.p.tt_node + c.e;

@@ -204,6 +204,11 @@ class Sim:
             self._stash.append(self._drain_now())
         return 0
 
+    def idle_jump(self, enable=True):
+        """ms_set_idle_jump: ms_run / ms_run_streamed / ms_recv jump over ticks at which no endpoint acts, with
+        byte-identical outputs; counters() counts only the rounds executed"""
+        return self._chk(self.L.ms_set_idle_jump(self.h, 1 if enable else 0))
+
     @property
     def now(self):
         return self.L.ms_now(self.h)
