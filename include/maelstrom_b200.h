@@ -328,6 +328,39 @@ int ms_net_set_loss(ms_sim* sim, double p);
  * cut.  Cleared by ms_net_heal. */
 int ms_net_partition(ms_sim* sim, const uint32_t* component_id, size_t n);
 
+/* Partition nemesis on the device (--nemesis partition, core.clj:60-80; DESIGN.md 2.13): one Jepsen partition
+ * schedule per cluster, applied inside the round loop.  Clusters: MS_W_RAFT the ms_config.reserved[4] blocks of g
+ * servers (0 = all), C = n_nodes / g whole clusters, servers past the last one never cut; any other workload one
+ * cluster of all servers.  Clients, host endpoints and services are never cut.
+ *   schedule  op j of cluster c draws x = Philox(j, c, 0x4E454D00, 0): t_j = t_{j-1} + ceil_tick((x0 * 2 interval)
+ *             >> 32), t_{-1} = start_ns; even j start a partition, odd j stop it.  An op takes effect before the
+ *             dequeues of the first round with now >= t_j; ops of one cluster due in one round apply in op order
+ *   targets   a start picks the enabled target (x1 * n_enabled) >> 32 of {one, majority, minority-third}; server
+ *             s of the cluster gets the key Philox(j, s, 0x4E454D01, 0) word 0, ranks by (key, s): ranks below
+ *             1 / g/2 + 1 / max(1, g/3) form side A (component 2c), the others side B (2c + 1); a healthy cluster's
+ *             servers are never cut.  (majorities-ring and primaries are not expressible as components)
+ *   end       no op with t_j >= time_limit_ns; at the first round with now >= time_limit_ns every partitioned
+ *             cluster gets a final stop
+ *   history   one ms_hist per op in ms_history_drain: client MS_H_NEMESIS, op j, value c, type MS_H_INFO,
+ *             f MS_HF_NEM_*, order round << 24 | 0xFFFFFF (after the round's client records)
+ * Once per simulation, start_ns >= ms_now; one GPU, no CUDA-graph replay, no bulk partition installed.  While it is
+ * on, ms_net_partition is MS_ERR_ARG and ms_net_heal also puts every server back to never-cut (the schedules go on:
+ * a healed cluster still gets its stop record). */
+typedef struct ms_nemesis_config {
+  uint32_t group;            /* servers per cluster: 0 = the workload's (reserved[4] for MS_W_RAFT, else all); <= 8192 */
+  uint32_t targets;          /* bit 0 one, bit 1 majority, bit 2 minority-third; 0 = all three */
+  int64_t  interval_ns;      /* --nemesis-interval: mean delay between two ops of a cluster; 0 = 10 s */
+  int64_t  start_ns;         /* t_{-1} */
+  int64_t  time_limit_ns;    /* --time-limit */
+} ms_nemesis_config;
+#define MS_H_NEMESIS 0xFFFFFFFFu
+enum { MS_HF_NEM_ONE = 5, MS_HF_NEM_MAJORITY = 6, MS_HF_NEM_MINORITY_THIRD = 7, MS_HF_NEM_STOP = 8 };
+int ms_set_nemesis(ms_sim* sim, const ms_nemesis_config* cfg);
+/* pure helper: the sides of start op `op` of cluster `cluster` (g servers) with target f = MS_HF_NEM_ONE /
+ * _MAJORITY / _MINORITY_THIRD under the seed: side_out[i] = 0 (side A) or 1 (side B) for server cluster * g + i */
+int ms_nemesis_grudge(uint32_t seed_lo, uint32_t seed_hi, uint32_t cluster, uint32_t g, uint32_t op, uint32_t target,
+                      uint32_t* side_out);
+
 /* ------------------------------------------------------------------ journal: jepsen-os + net.journal */
 /* j/journal + j/close! (net.clj:128-137): stream drained events to a file.  A path ending in
  * ".fressian" gets the reference's own format -- Fressian `Event{id time type message}` objects as

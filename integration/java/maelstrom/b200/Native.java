@@ -40,6 +40,8 @@ public final class Native {
   public static native int netFlaky(long h);
   public static native int netSetLoss(long h, double p);
   public static native int netPartition(long h, ByteBuffer componentIds, long n);
+  public static native int setNemesis(long h, ByteBuffer msNemesisConfig);
+  public static native int nemesisGrudge(int seedLo, int seedHi, int cluster, int g, int op, int target, ByteBuffer sides);
   public static native int journalOpen(long h, String path);
   public static native int journalClose(long h);
   public static native long journalDrain(long h, ByteBuffer events, ByteBuffer bodies, long cap);

@@ -55,6 +55,11 @@ class KvGenConfig(C.Structure):   # ms_kv_gen_config
                 ("key_period_ns", C.c_int64)]
 
 
+class NemesisConfig(C.Structure):   # ms_nemesis_config
+    _fields_ = [("group", C.c_uint32), ("targets", C.c_uint32), ("interval_ns", C.c_int64), ("start_ns", C.c_int64),
+                ("time_limit_ns", C.c_int64)]
+
+
 HIST_DTYPE = np.dtype([("time_ns", "<i8"), ("order", "<u8"), ("client", "<u4"), ("op", "<u4"), ("type", "u1"),
                        ("f", "u1"), ("error", "<u2"), ("value", "<u4")])
 assert HIST_DTYPE.itemsize == 32
@@ -103,6 +108,8 @@ SYMBOLS = {
     "ms_net_flaky": (C.c_int, [_P]),
     "ms_net_set_loss": (C.c_int, [_P, C.c_double]),
     "ms_net_partition": (C.c_int, [_P, _P, C.c_size_t]),
+    "ms_set_nemesis": (C.c_int, [_P, _P]),
+    "ms_nemesis_grudge": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, _P]),
     "ms_journal_open": (C.c_int, [_P, C.c_char_p]),
     "ms_journal_close": (C.c_int, [_P]),
     "ms_journal_drain": (C.c_int, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t)]),

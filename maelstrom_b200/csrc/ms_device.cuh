@@ -78,6 +78,9 @@ struct DevState {
   // idle-time jump (ms_set_idle_jump): ~(earliest instant at which an endpoint acts), folded in by k_wake with
   // atomicMax (a minimum of the instant), 0 = none; consumed and cleared by k_jump.  Appended: nothing moves
   uint64_t idle_wake;
+  // partition nemesis (ms_set_nemesis): the earliest instant at which some cluster acts (nem_pending); k_nemesis
+  // returns at once before it.  Appended
+  int64_t  nem_next;
 };
 
 // One row per round, kept in a ring of `hist` rounds: what is needed to turn an
@@ -247,6 +250,10 @@ struct Params {
   // Appended, so that nothing the other kernels read from Params moves
   uint32_t  kv_value_range, kv_keys_per_group;
   int64_t   kv_key_period_ns;
+  // partition nemesis (ms_set_nemesis, csrc/ms_nemesis.h): per-cluster state, nullptr = off.  Appended
+  struct NemDev* nem;
+  uint32_t  nem_clusters, nem_group, nem_targets, nem_pad;
+  int64_t   nem_interval_ns, nem_limit_ns;
 };
 
 constexpr uint32_t kRaftCallbacks = 4096;       // default pending-RPC table slots per node (ms_config.reserved[5]; oracle: same)

@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "ms_device.cuh"
+#include "ms_nemesis.h"
 #include "ms_tree.h"
 #include "ms_fressian.h"
 #include "ms_json.h"
@@ -33,6 +34,7 @@ void msk_launch_round(const msd::Params* p, int n_classes, const uint32_t* caps,
 void msk_set_bit(uint32_t* words, size_t word, uint32_t bit, cudaStream_t s);
 void msk_barrier(const msd::Params* p, cudaStream_t s);
 void msk_launch_idle_jump(const msd::Params* p, cudaStream_t s);
+void msk_launch_nemesis(const msd::Params* p, cudaStream_t s);
 void msk_journal_expand(const msd::Params* p, uint64_t r0, uint32_t n_rounds, uint64_t first, uint64_t count,
                         void* out_ev, void* out_body, int n_sms, cudaStream_t s);
 size_t msk_stream_plan_bytes();
@@ -238,6 +240,28 @@ struct ms_sim {
     return MS_OK;
   }
 
+  // The ring of ms_hist records shared by the closed-loop clients and the nemesis: at least `cap` records; a
+  // bigger ring keeps the records not drained yet at their positions
+  int hist_ring(uint32_t cap) {
+    if (P.gc_hist && P.gc_hist_mask + 1u >= cap) return MS_OK;
+    uint4* ring = nullptr;
+    int rc;
+    if ((rc = dalloc(&ring, (size_t)cap * 2))) return rc;
+    if (P.gc_hist) {
+      CK(cudaStreamSynchronize(stream));
+      std::vector<uint4> old((size_t)(P.gc_hist_mask + 1u) * 2), now((size_t)cap * 2);
+      CK(cudaMemcpy(old.data(), P.gc_hist, old.size() * 16, cudaMemcpyDeviceToHost));
+      for (uint64_t pos = hs.gc_hist_drained; pos < hs.gc_hist_n; pos++)
+        for (int v = 0; v < 2; v++) now[(pos & (cap - 1u)) * 2 + v] = old[(pos & P.gc_hist_mask) * 2 + v];
+      CK(cudaMemcpy(ring, now.data(), now.size() * 16, cudaMemcpyHostToDevice));
+      allocs.erase(std::find(allocs.begin(), allocs.end(), (void*)P.gc_hist));
+      CK(cudaFree(P.gc_hist));
+    }
+    P.gc_hist = ring;
+    P.gc_hist_mask = cap - 1u;
+    return MS_OK;
+  }
+
   int push_np() {
     CK(cudaMemcpyAsync(P.np, &np, sizeof(np), cudaMemcpyHostToDevice, stream));
     return MS_OK;
@@ -260,8 +284,12 @@ struct ms_sim {
     }
     if (hs.error) {
       char buf[256];
-      snprintf(buf, sizeof buf, "%s %u (round %llu)", dev_error_text(hs.error), hs.error_arg,
-               (unsigned long long)hs.round);
+      if (hs.error == E_HISTORY_RING && hs.error_arg == MS_H_NEMESIS)   // latched by k_nemesis, not by a client
+        snprintf(buf, sizeof buf, "history ring is full of undrained records (call ms_history_drain more often) at a "
+                 "nemesis op (round %llu)", (unsigned long long)hs.round);
+      else
+        snprintf(buf, sizeof buf, "%s %u (round %llu)", dev_error_text(hs.error), hs.error_arg,
+                 (unsigned long long)hs.round);
       set_err(buf);
       return MS_ERR_SIM;
     }
@@ -341,6 +369,10 @@ struct ms_sim {
         if (jump) {
           msk_launch_idle_jump(&P, stream);
           if (!capturing()) launches += 2;
+        }
+        if (P.nem) {          // after the jump: the nemesis acts in the round the jump lands on
+          msk_launch_nemesis(&P, stream);
+          if (!capturing()) launches += 1;
         }
         msk_launch_round(&P, n_classes, class_cap, class_threads, grids, use_calendar ? 1 : 0, stream, a, b, 15, aux_streams, aux_events);
         if (!capturing()) launches += (use_calendar ? 2 : 1) + n_classes + (P.split_commit ? (P.cm_blk ? 3 : 1) : 0);
@@ -1045,8 +1077,7 @@ int ms_add_gen_clients(ms_sim* s, const ms_gen_config* gc, uint32_t first_name) 
   Params& P = s->P;
   int rc;
   const uint32_t hist_cap = pow2_at_least(std::max<uint32_t>(1u << 16, 64u * gc->n_clients));
-  if ((rc = s->dalloc(&P.gc, s->cfg.max_endpoints)) || (rc = s->dalloc(&P.gc_hist, (size_t)hist_cap * 2))) return rc;
-  P.gc_hist_mask = hist_cap - 1u;
+  if ((rc = s->dalloc(&P.gc, s->cfg.max_endpoints)) || (rc = s->hist_ring(hist_cap))) return rc;
   P.gc_n = gc->n_clients;
   P.gc_read_permille = gc->read_permille;
   P.gc_interval_ns = gc->interval_ns;
@@ -1105,8 +1136,7 @@ int ms_add_kv_clients(ms_sim* s, const ms_kv_gen_config* kc, uint32_t first_name
     if (s->by_name.count("c" + std::to_string(first_name + k))) { set_err("endpoint already exists: c" + std::to_string(first_name + k)); return MS_ERR_ARG; }
   int rc;
   const uint32_t hist_cap = pow2_at_least(std::max<uint32_t>(1u << 16, 64u * kc->n_clients));
-  if ((rc = s->dalloc(&P.gc, s->cfg.max_endpoints)) || (rc = s->dalloc(&P.gc_hist, (size_t)hist_cap * 2))) return rc;
-  P.gc_hist_mask = hist_cap - 1u;
+  if ((rc = s->dalloc(&P.gc, s->cfg.max_endpoints)) || (rc = s->hist_ring(hist_cap))) return rc;
   P.gc_n = kc->n_clients;
   P.gc_interval_ns = kc->interval_ns;
   P.gc_timeout_ns = kc->timeout_ns > 0 ? kc->timeout_ns
@@ -1537,7 +1567,10 @@ int ms_net_heal(ms_sim* s) {
   if (s->pair_alloc && s->np.pair_active)
     CK(cudaMemsetAsync(s->P.pair_bits, 0, (size_t)s->cfg.max_endpoints * s->P.pair_words * 4, s->stream));
   s->np.pair_active = 0;
-  s->np.comp_active = 0;
+  if (s->P.nem)        // the nemesis keeps the component vector: every server back to never-cut, the schedules go on
+    CK(cudaMemsetAsync(s->P.comp, 0xFF, (size_t)s->cfg.max_endpoints * 4, s->stream));
+  else
+    s->np.comp_active = 0;
   return s->push_np();
 }
 
@@ -1575,6 +1608,7 @@ int ms_net_partition(ms_sim* s, const uint32_t* comp, size_t n) {
   std::lock_guard<std::mutex> g(s->mu);
   cudaSetDevice(s->device);
   if (n > s->cfg.max_endpoints) { set_err("partition vector longer than max_endpoints"); return MS_ERR_ARG; }
+  if (s->P.nem) { set_err("ms_net_partition: the nemesis owns the component vector (ms_set_nemesis)"); return MS_ERR_ARG; }
   std::vector<uint32_t> full(s->cfg.max_endpoints, 0);
   // endpoints not listed (index >= n) carry 0xFFFFFFFF = "never cut" (clients keep talking to every node)
   for (size_t i = 0; i < n; i++) full[i] = comp[i];
@@ -1582,6 +1616,71 @@ int ms_net_partition(ms_sim* s, const uint32_t* comp, size_t n) {
   CK(cudaMemcpy(s->P.comp, full.data(), full.size() * 4, cudaMemcpyHostToDevice));
   s->np.comp_active = 1;
   return s->push_np();
+}
+
+// Partition nemesis (DESIGN.md 2.13): per-cluster schedules run by k_nemesis before every executed round.
+int ms_set_nemesis(ms_sim* s, const ms_nemesis_config* nc) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  Params& P = s->P;
+  if (!nc) { set_err("ms_set_nemesis: null configuration"); return MS_ERR_ARG; }
+  if (P.nem) { set_err("ms_set_nemesis: the nemesis is on already (once per simulation)"); return MS_ERR_ARG; }
+  if (P.n_shards > 1) { set_err("ms_set_nemesis: single GPU only"); return MS_ERR_ARG; }
+  if (s->cfg.reserved[1] == 1) { set_err("ms_set_nemesis: not with CUDA-graph replay (ms_config.reserved[1] = 1)"); return MS_ERR_ARG; }
+  if (s->np.comp_active) { set_err("ms_set_nemesis: a bulk partition is installed (ms_net_heal first)"); return MS_ERR_ARG; }
+  const uint32_t N = s->cfg.n_nodes;
+  const uint32_t natural = (s->cfg.workload == MS_W_RAFT && P.rf_group) ? P.rf_group : N;
+  const uint32_t gsz = nc->group ? nc->group : natural;
+  if (gsz != natural || gsz == 0 || gsz > kNemMaxGroup) {
+    set_err("ms_set_nemesis: bad group (the workload's clusters have " + std::to_string(natural) +
+            " servers; broadcast gossip crosses any smaller grouping; at most 8192)");
+    return MS_ERR_ARG;
+  }
+  if (nc->targets & ~7u) { set_err("ms_set_nemesis: bad target mask"); return MS_ERR_ARG; }
+  const int64_t interval = nc->interval_ns ? nc->interval_ns : kNemDefaultIntervalNs;
+  if (interval < 0 || interval > kNemMaxIntervalNs) { set_err("ms_set_nemesis: bad interval"); return MS_ERR_ARG; }
+  if (nc->start_ns < s->hs.now) { set_err("ms_set_nemesis: start_ns is in the past"); return MS_ERR_ARG; }
+  const uint32_t C = N / gsz;
+  int rc;
+  std::vector<NemDev> init(C);
+  int64_t next = INT64_MAX;
+  for (uint32_t c = 0; c < C; c++) {
+    uint32_t x[4];
+    nem_draw(P.seed_lo, P.seed_hi, c, 0, x);
+    init[c].t = nem_add(nc->start_ns, nem_delay_ns(x[0], interval));
+    init[c].op = 0;
+    init[c].part = 0;
+    next = std::min(next, nem_pending(init[c], nc->time_limit_ns));
+  }
+  NemDev* nem = nullptr;
+  if ((rc = s->hist_ring(pow2_at_least(std::max<uint32_t>(1u << 16, 64u * C)))) || (rc = s->dalloc(&nem, C))) return rc;
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(nem, init.data(), init.size() * sizeof(NemDev), cudaMemcpyHostToDevice));
+  CK(cudaMemset(P.comp, 0xFF, (size_t)s->cfg.max_endpoints * 4));
+  CK(cudaMemcpy(&P.st->nem_next, &next, sizeof(next), cudaMemcpyHostToDevice));
+  s->hs.nem_next = next;
+  P.nem = nem;
+  P.nem_clusters = C;
+  P.nem_group = gsz;
+  P.nem_targets = nc->targets;
+  P.nem_interval_ns = interval;
+  P.nem_limit_ns = nc->time_limit_ns;
+  s->np.comp_active = 1;
+  return s->push_np();
+}
+
+int ms_nemesis_grudge(uint32_t seed_lo, uint32_t seed_hi, uint32_t cluster, uint32_t g, uint32_t op, uint32_t target,
+                      uint32_t* side_out) {
+  if (!side_out || g == 0 || g > kNemMaxGroup || target < MS_HF_NEM_ONE || target > MS_HF_NEM_MINORITY_THIRD ||
+      (uint64_t)cluster * g + g > 0xFFFFFFFFull) {
+    set_err("ms_nemesis_grudge: bad arguments");
+    return MS_ERR_ARG;
+  }
+  std::vector<uint32_t> keys(g);
+  for (uint32_t k = 0; k < g; k++) keys[k] = nem_key(seed_lo, seed_hi, op, cluster * g + k);
+  const uint32_t m = nem_side_a(target, g);
+  for (uint32_t k = 0; k < g; k++) side_out[k] = nem_rank(keys.data(), g, k) < m ? 0u : 1u;
+  return MS_OK;
 }
 
 int ms_journal_open(ms_sim* s, const char* path) {

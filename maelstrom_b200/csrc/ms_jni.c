@@ -124,6 +124,17 @@ jint FN(netPartition)(JNIEnv* env, jclass c, jlong h, jobject comp, jlong n) {
   (void)c;
   return ms_net_partition(H(h), (const uint32_t*)BUF(comp), (size_t)n);
 }
+/* partition nemesis: cfg = direct buffer holding an ms_nemesis_config; sides = direct buffer of g uint32 */
+jint FN(setNemesis)(JNIEnv* env, jclass c, jlong h, jobject cfg) {
+  (void)c;
+  return ms_set_nemesis(H(h), (const ms_nemesis_config*)BUF(cfg));
+}
+jint FN(nemesisGrudge)(JNIEnv* env, jclass c, jint seedLo, jint seedHi, jint cluster, jint g, jint op, jint target,
+                       jobject sides) {
+  (void)c;
+  return ms_nemesis_grudge((uint32_t)seedLo, (uint32_t)seedHi, (uint32_t)cluster, (uint32_t)g, (uint32_t)op,
+                           (uint32_t)target, (uint32_t*)BUF(sides));
+}
 
 /* journal (net.clj:128-137, net/journal.clj:205-239) */
 jint FN(journalOpen)(JNIEnv* env, jclass c, jlong h, jstring path) {

@@ -31,6 +31,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "ms_device.cuh"
+#include "ms_nemesis.h"
 
 namespace msd {
 
@@ -798,11 +799,111 @@ __global__ void k_wake(Params p) {
     const int64_t t = p.sched[st->sched_cursor].time_ns;
     w = min(w, t <= 0 ? (int64_t)0 : ((t + kTickNs - 1) / kTickNs) * kTickNs);
   }
+  // k_nemesis: the earliest instant at which some cluster's op (or final stop) is due
+  if (gid == 0 && p.nem) w = min(w, st->nem_next);
   if (w < now) w = now;
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) w = min(w, (int64_t)__shfl_xor_sync(FULL, w, d));
   if ((threadIdx.x & 31) == 0 && w != INT64_MAX)
     atomicMax((unsigned long long*)&st->idle_wake, (unsigned long long)~(uint64_t)w);
+}
+
+// ------------------------------------------------------------------ k_nemesis (ms_set_nemesis, DESIGN.md 2.13)
+// One CTA before every executed round while the nemesis is on: returns at once unless `now` has reached the
+// earliest pending instant; otherwise performs every due op of every cluster, in (cluster, op) order -- the
+// component ids of the cluster's servers in p.comp and one history record per op -- and recomputes that instant.
+constexpr int kNemThreads = 512;
+__global__ void __launch_bounds__(kNemThreads) k_nemesis(Params p) {
+  __shared__ uint32_t s_key[kNemMaxGroup];
+  __shared__ uint32_t s_due[kNemThreads];
+  __shared__ uint32_t s_wcnt[kNemThreads / 32];
+  __shared__ int64_t  s_wmin[kNemThreads / 32];
+  __shared__ NemDev   s_nd;
+  __shared__ uint32_t s_act;                           // 0 nothing more due, else the op's MS_HF_NEM_* code
+  DevState* st = p.st;
+  if (round_skipped(p, st) || st->now < st->nem_next) return;
+  const int64_t now = st->now;
+  const uint64_t round = st->round;
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, nw = blockDim.x >> 5;
+  const uint32_t g = p.nem_group;
+  __syncthreads();   // every thread has read the state before thread 0 changes it
+  for (uint32_t c0 = 0; c0 < p.nem_clusters; c0 += blockDim.x) {
+    // the due clusters of this stretch, in cluster order
+    const uint32_t cc = c0 + tid;
+    const bool due = cc < p.nem_clusters && nem_pending(p.nem[cc], p.nem_limit_ns) <= now;
+    const uint32_t b = __ballot_sync(FULL, due);
+    if (lane == 0) s_wcnt[warp] = __popc(b);
+    __syncthreads();
+    uint32_t off = 0, n_due = 0;
+    for (uint32_t w = 0; w < nw; w++) { off += w < warp ? s_wcnt[w] : 0u; n_due += s_wcnt[w]; }
+    if (due) s_due[off + __popc(b & ((1u << lane) - 1u))] = cc;
+    __syncthreads();
+    for (uint32_t i = 0; i < n_due; i++) {
+      const uint32_t c = s_due[i];
+      if (tid == 0) s_nd = p.nem[c];
+      for (;;) {
+        __syncthreads();
+        if (tid == 0) {
+          uint32_t act = 0;
+          if (s_nd.t < p.nem_limit_ns) {
+            if (s_nd.t <= now) {
+              uint32_t x[4];
+              nem_draw(p.seed_lo, p.seed_hi, c, s_nd.op, x);
+              act = (s_nd.op & 1u) ? (uint32_t)MS_HF_NEM_STOP : nem_target(p.nem_targets, x[1]);
+            }
+          } else if (s_nd.part && now >= p.nem_limit_ns) {
+            act = MS_HF_NEM_STOP;                      // the final generator (core.clj:72-76)
+          }
+          s_act = act;
+        }
+        __syncthreads();
+        const uint32_t act = s_act;
+        if (act == 0) break;
+        const uint32_t op = s_nd.op, base = c * g;
+        if (act != MS_HF_NEM_STOP) {
+          for (uint32_t k = tid; k < g; k += blockDim.x) s_key[k] = nem_key(p.seed_lo, p.seed_hi, op, base + k);
+          __syncthreads();
+          const uint32_t m = nem_side_a(act, g);
+          for (uint32_t k = tid; k < g; k += blockDim.x) p.comp[base + k] = nem_rank(s_key, g, k) < m ? 2u * c : 2u * c + 1u;
+        } else {
+          for (uint32_t k = tid; k < g; k += blockDim.x) p.comp[base + k] = 0xFFFFFFFFu;
+        }
+        __syncthreads();   // s_key is rewritten by the next op
+        if (tid == 0) {
+          const unsigned long long pos = atomicAdd((unsigned long long*)&st->gc_hist_n, 1ull);
+          if (pos - st->gc_hist_drained > p.gc_hist_mask) {
+            latch_error(st, E_HISTORY_RING, MS_H_NEMESIS);
+          } else {
+            uint4* at = p.gc_hist + (pos & p.gc_hist_mask) * 2;
+            const uint64_t order = (round << 24) | 0xFFFFFFull;
+            at[0] = make_uint4((uint32_t)now, (uint32_t)((uint64_t)now >> 32), (uint32_t)order, (uint32_t)(order >> 32));
+            at[1] = make_uint4(MS_H_NEMESIS, op, (uint32_t)MS_H_INFO | (act << 8), c);
+          }
+          s_nd.part = act != MS_HF_NEM_STOP;
+          s_nd.op = op + 1;
+          if (s_nd.t < p.nem_limit_ns) {
+            uint32_t x[4];
+            nem_draw(p.seed_lo, p.seed_hi, c, op + 1, x);
+            s_nd.t = nem_add(s_nd.t, nem_delay_ns(x[0], p.nem_interval_ns));
+          }
+        }
+      }
+      if (tid == 0) p.nem[c] = s_nd;
+    }
+    __syncthreads();   // s_due / s_wcnt are rewritten by the next stretch
+  }
+  __syncthreads();
+  int64_t w = INT64_MAX;
+  for (uint32_t c = tid; c < p.nem_clusters; c += blockDim.x) w = min(w, nem_pending(p.nem[c], p.nem_limit_ns));
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) w = min(w, (int64_t)__shfl_xor_sync(FULL, w, d));
+  if (lane == 0) s_wmin[warp] = w;
+  __syncthreads();
+  if (tid == 0) {
+    for (uint32_t k = 1; k < nw; k++) w = min(w, s_wmin[k]);
+    st->nem_next = w;
+    __threadfence();
+  }
 }
 
 // ------------------------------------------------------------------ k_release (timing wheel -> rings)
@@ -2920,6 +3021,8 @@ void msk_launch_idle_jump(const msd::Params* p, cudaStream_t s) {
   MS_LAUNCH(msd::k_wake, g, 256, 0, s, *p);
   MS_LAUNCH(msd::k_jump, 1, 512, 0, s, *p);
 }
+
+void msk_launch_nemesis(const msd::Params* p, cudaStream_t s) { MS_LAUNCH(msd::k_nemesis, 1, msd::kNemThreads, 0, s, *p); }
 
 size_t msk_stream_plan_bytes() { return sizeof(msd::StreamPlan); }
 // plan -> pack -> finish: one batch of the journal into (host-mapped) `out`, header into `hdr`

@@ -240,6 +240,14 @@ class Sim:
         comp = np.ascontiguousarray(comp, dtype=np.uint32)
         return self._chk(self.L.ms_net_partition(self.h, comp.ctypes.data, comp.size))
 
+    def nemesis(self, time_limit_ns, interval_ns=0, start_ns=None, targets=0, group=0):
+        """ms_set_nemesis: a Jepsen partition schedule per cluster, run on the device before every round (DESIGN.md
+        2.13).  targets: a mask of NEM_ONE / NEM_MAJORITY / NEM_MINORITY_THIRD (0 = all three); interval_ns 0 = 10 s;
+        start_ns None = now (an earlier instant is refused); group 0 = the workload's clusters.  Each op is a
+        history() record with client H_NEMESIS"""
+        nc = _lib.NemesisConfig(group, targets, interval_ns, self.now if start_ns is None else start_ns, time_limit_ns)
+        return self._chk(self.L.ms_set_nemesis(self.h, C.byref(nc)))
+
     # journal -------------------------------------------------------------
     def journal_open(self, path):
         return self._chk(self.L.ms_journal_open(self.h, path.encode()))
@@ -412,6 +420,20 @@ class Sim:
 
 HIST_TYPES = ("invoke", "ok", "fail", "info")              # MS_H_*
 HF_KV_READ, HF_KV_WRITE, HF_KV_CAS = 2, 3, 4              # MS_HF_KV_*
+H_NEMESIS = 0xFFFFFFFF                                    # MS_H_NEMESIS: the client of a nemesis record
+HF_NEM_ONE, HF_NEM_MAJORITY, HF_NEM_MINORITY_THIRD, HF_NEM_STOP = 5, 6, 7, 8   # MS_HF_NEM_*
+NEM_ONE, NEM_MAJORITY, NEM_MINORITY_THIRD = 1, 2, 4       # ms_nemesis_config.targets bits
+
+
+def nemesis_grudge(seed, cluster, g, op, target):
+    """ms_nemesis_grudge: the sides of a nemesis start record (op = its op, target = its f, cluster = its value) in a
+    simulation with this seed and g servers per cluster; uint32 array, entry i = 0 (side A) / 1 (side B) for server
+    cluster * g + i"""
+    out = np.zeros(max(g, 1), dtype=np.uint32)
+    rc = _lib.lib().ms_nemesis_grudge(seed & 0xFFFFFFFF, seed >> 32, cluster, g, op, target, out.ctypes.data)
+    if rc < 0:
+        raise SimError(rc, _lib.lib().ms_last_error(None).decode())
+    return out[:g]
 
 
 def kv_history(records, first_client, group_clients):
@@ -420,9 +442,11 @@ def kv_history(records, first_client, group_clients):
     one per register -- a group works on one cluster, so equal keys of different groups are different
     registers.  Each op is {"process", "type", "f", "value", "time", "error"} in Jepsen's shape for independent
     keys: value (k, v) for a read (v None unless it is an :ok) and a write, (k, (from, to)) for a cas;
-    process = the client's endpoint index."""
+    process = the client's endpoint index.  Nemesis records (client H_NEMESIS) are left out."""
     out = {}
     for r in records:
+        if int(r["client"]) == H_NEMESIS:
+            continue
         f, v = int(r["f"]), int(r["value"])
         k, a, b = v & 0xFFFF, (v >> 16) & 0xFF, v >> 24
         if f == HF_KV_READ:
