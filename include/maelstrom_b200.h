@@ -335,29 +335,40 @@ int ms_net_partition(ms_sim* sim, const uint32_t* component_id, size_t n);
  *   schedule  op j of cluster c draws x = Philox(j, c, 0x4E454D00, 0): t_j = t_{j-1} + ceil_tick((x0 * 2 interval)
  *             >> 32), t_{-1} = start_ns; even j start a partition, odd j stop it.  An op takes effect before the
  *             dequeues of the first round with now >= t_j; ops of one cluster due in one round apply in op order
- *   targets   a start picks the enabled target (x1 * n_enabled) >> 32 of {one, majority, minority-third}; server
- *             s of the cluster gets the key Philox(j, s, 0x4E454D01, 0) word 0, ranks by (key, s): ranks below
- *             1 / g/2 + 1 / max(1, g/3) form side A (component 2c), the others side B (2c + 1); a healthy cluster's
- *             servers are never cut.  (majorities-ring and primaries are not expressible as components)
+ *   targets   a start picks the enabled target (x1 * n_enabled) >> 32 of {one, majority, minority-third,
+ *             majorities-ring}; server s of the cluster gets the key Philox(j, s, 0x4E454D01, 0) word 0, its ring
+ *             position p_s is its rank by (key, s).  one / majority / minority-third: positions below 1 / g/2 + 1 /
+ *             max(1, g/3) form side A (component 2c), the others side B (2c + 1).  majorities-ring: with m = g/2 + 1
+ *             and h = m/2, the server at position p receives from the one at position q iff (q - p + h) mod g < m;
+ *             every other message between two servers of the cluster is cut at dequeue, like drop!(src, dest), in
+ *             the cluster's block of the pairwise matrix (its comp entries stay never-cut).  A healthy cluster's
+ *             servers are never cut.  (primaries is not offered: the Maelstrom db has no primaries)
  *   end       no op with t_j >= time_limit_ns; at the first round with now >= time_limit_ns every partitioned
  *             cluster gets a final stop
  *   history   one ms_hist per op in ms_history_drain: client MS_H_NEMESIS, op j, value c, type MS_H_INFO,
  *             f MS_HF_NEM_*, order round << 24 | 0xFFFFFF (after the round's client records)
  * Once per simulation, start_ns >= ms_now; one GPU, no CUDA-graph replay, no bulk partition installed.  While it is
  * on, ms_net_partition is MS_ERR_ARG and ms_net_heal also puts every server back to never-cut (the schedules go on:
- * a healed cluster still gets its stop record). */
+ * a healed cluster still gets its stop record).  With majorities-ring enabled the nemesis also owns the pairwise
+ * matrix: it needs max_endpoints <= 65536 (else MS_ERR_CAPACITY, as drop!) and no drop! installed, drop! is
+ * MS_ERR_ARG, and drop!'s endpoint-slot rule holds for the rest of the simulation (removed clients' slots are not
+ * recycled). */
 typedef struct ms_nemesis_config {
   uint32_t group;            /* servers per cluster: 0 = the workload's (reserved[4] for MS_W_RAFT, else all); <= 8192 */
-  uint32_t targets;          /* bit 0 one, bit 1 majority, bit 2 minority-third; 0 = all three */
+  uint32_t targets;          /* bit 0 one, bit 1 majority, bit 2 minority-third, bit 4 majorities-ring (bit 3,
+                                primaries, and bits above 4 are MS_ERR_ARG); 0 = the first three */
   int64_t  interval_ns;      /* --nemesis-interval: mean delay between two ops of a cluster; 0 = 10 s */
   int64_t  start_ns;         /* t_{-1} */
   int64_t  time_limit_ns;    /* --time-limit */
 } ms_nemesis_config;
 #define MS_H_NEMESIS 0xFFFFFFFFu
-enum { MS_HF_NEM_ONE = 5, MS_HF_NEM_MAJORITY = 6, MS_HF_NEM_MINORITY_THIRD = 7, MS_HF_NEM_STOP = 8 };
+enum { MS_HF_NEM_ONE = 5, MS_HF_NEM_MAJORITY = 6, MS_HF_NEM_MINORITY_THIRD = 7, MS_HF_NEM_STOP = 8,
+       MS_HF_NEM_MAJORITIES_RING = 9 };
 int ms_set_nemesis(ms_sim* sim, const ms_nemesis_config* cfg);
-/* pure helper: the sides of start op `op` of cluster `cluster` (g servers) with target f = MS_HF_NEM_ONE /
- * _MAJORITY / _MINORITY_THIRD under the seed: side_out[i] = 0 (side A) or 1 (side B) for server cluster * g + i */
+/* pure helper: the grudge of start op `op` of cluster `cluster` (g servers) with target f under the seed, for server
+ * cluster * g + i.  f = MS_HF_NEM_ONE / _MAJORITY / _MINORITY_THIRD: side_out[i] = 0 (side A) or 1 (side B).
+ * f = MS_HF_NEM_MAJORITIES_RING: side_out[i] = the server's ring position p; the server at position p receives from
+ * the one at q iff (q - p + h) mod g < m, m = g/2 + 1, h = m/2 */
 int ms_nemesis_grudge(uint32_t seed_lo, uint32_t seed_hi, uint32_t cluster, uint32_t g, uint32_t op, uint32_t target,
                       uint32_t* side_out);
 

@@ -262,6 +262,18 @@ struct ms_sim {
     return MS_OK;
   }
 
+  // The [dest][src] bit matrix of pairwise cuts (drop!, the majorities-ring nemesis), allocated on first use
+  int pair_matrix() {
+    if (pair_alloc) return MS_OK;
+    const uint32_t M = cfg.max_endpoints;
+    if (M > 65536) { set_err("pairwise drop! needs max_endpoints <= 65536; use ms_net_partition"); return MS_ERR_CAPACITY; }
+    P.pair_words = (M + 31) / 32;
+    int rc = dalloc(&P.pair_bits, (size_t)M * P.pair_words);
+    if (rc) return rc;
+    pair_alloc = true;
+    return MS_OK;
+  }
+
   int push_np() {
     CK(cudaMemcpyAsync(P.np, &np, sizeof(np), cudaMemcpyHostToDevice, stream));
     return MS_OK;
@@ -1549,13 +1561,11 @@ int ms_net_drop(ms_sim* s, uint32_t src, uint32_t dest) {
   cudaSetDevice(s->device);
   const uint32_t M = s->cfg.max_endpoints;
   if (src >= M || dest >= M) { set_err("drop!: endpoint out of range"); return MS_ERR_ARG; }
-  if (!s->pair_alloc) {
-    if (M > 65536) { set_err("pairwise drop! needs max_endpoints <= 65536; use ms_net_partition"); return MS_ERR_CAPACITY; }
-    s->P.pair_words = (M + 31) / 32;
-    int rc = s->dalloc(&s->P.pair_bits, (size_t)M * s->P.pair_words);
-    if (rc) return rc;
-    s->pair_alloc = true;
+  if (s->P.nem && (s->P.nem_targets & kNemRingTarget)) {
+    set_err("drop!: the majorities-ring nemesis owns the pairwise matrix (ms_set_nemesis)");
+    return MS_ERR_ARG;
   }
+  if (int rc = s->pair_matrix()) return rc;
   msk_set_bit(s->P.pair_bits, (size_t)dest * s->P.pair_words + (src >> 5), src & 31, s->stream);
   s->np.pair_active = 1;
   return s->push_np();
@@ -1566,7 +1576,8 @@ int ms_net_heal(ms_sim* s) {
   cudaSetDevice(s->device);
   if (s->pair_alloc && s->np.pair_active)
     CK(cudaMemsetAsync(s->P.pair_bits, 0, (size_t)s->cfg.max_endpoints * s->P.pair_words * 4, s->stream));
-  s->np.pair_active = 0;
+  // the majorities-ring nemesis keeps the matrix switched on: its clusters' blocks are cut again by later starts
+  s->np.pair_active = s->P.nem && (s->P.nem_targets & kNemRingTarget) ? 1 : 0;
   if (s->P.nem)        // the nemesis keeps the component vector: every server back to never-cut, the schedules go on
     CK(cudaMemsetAsync(s->P.comp, 0xFF, (size_t)s->cfg.max_endpoints * 4, s->stream));
   else
@@ -1636,7 +1647,16 @@ int ms_set_nemesis(ms_sim* s, const ms_nemesis_config* nc) {
             " servers; broadcast gossip crosses any smaller grouping; at most 8192)");
     return MS_ERR_ARG;
   }
-  if (nc->targets & ~7u) { set_err("ms_set_nemesis: bad target mask"); return MS_ERR_ARG; }
+  if (nc->targets & 8u) {
+    set_err("ms_set_nemesis: target bit 3 (primaries) is not offered: the Maelstrom db has no primaries");
+    return MS_ERR_ARG;
+  }
+  if (nc->targets & ~kNemTargetBits) { set_err("ms_set_nemesis: bad target mask"); return MS_ERR_ARG; }
+  const bool ring = nc->targets & kNemRingTarget;
+  if (ring && s->np.pair_active) {
+    set_err("ms_set_nemesis: drop! entries are installed and majorities-ring needs the pairwise matrix (ms_net_heal first)");
+    return MS_ERR_ARG;
+  }
   const int64_t interval = nc->interval_ns ? nc->interval_ns : kNemDefaultIntervalNs;
   if (interval < 0 || interval > kNemMaxIntervalNs) { set_err("ms_set_nemesis: bad interval"); return MS_ERR_ARG; }
   if (nc->start_ns < s->hs.now) { set_err("ms_set_nemesis: start_ns is in the past"); return MS_ERR_ARG; }
@@ -1653,6 +1673,7 @@ int ms_set_nemesis(ms_sim* s, const ms_nemesis_config* nc) {
     next = std::min(next, nem_pending(init[c], nc->time_limit_ns));
   }
   NemDev* nem = nullptr;
+  if (ring && (rc = s->pair_matrix())) return rc;   // all zero: allocated here or cleared by the last heal
   if ((rc = s->hist_ring(pow2_at_least(std::max<uint32_t>(1u << 16, 64u * C)))) || (rc = s->dalloc(&nem, C))) return rc;
   CK(cudaStreamSynchronize(s->stream));
   CK(cudaMemcpy(nem, init.data(), init.size() * sizeof(NemDev), cudaMemcpyHostToDevice));
@@ -1666,12 +1687,14 @@ int ms_set_nemesis(ms_sim* s, const ms_nemesis_config* nc) {
   P.nem_interval_ns = interval;
   P.nem_limit_ns = nc->time_limit_ns;
   s->np.comp_active = 1;
+  if (ring) s->np.pair_active = 1;   // for the rest of the simulation, ms_net_heal included
   return s->push_np();
 }
 
 int ms_nemesis_grudge(uint32_t seed_lo, uint32_t seed_hi, uint32_t cluster, uint32_t g, uint32_t op, uint32_t target,
                       uint32_t* side_out) {
-  if (!side_out || g == 0 || g > kNemMaxGroup || target < MS_HF_NEM_ONE || target > MS_HF_NEM_MINORITY_THIRD ||
+  const bool ring = target == MS_HF_NEM_MAJORITIES_RING;
+  if (!side_out || g == 0 || g > kNemMaxGroup || ((target < MS_HF_NEM_ONE || target > MS_HF_NEM_MINORITY_THIRD) && !ring) ||
       (uint64_t)cluster * g + g > 0xFFFFFFFFull) {
     set_err("ms_nemesis_grudge: bad arguments");
     return MS_ERR_ARG;
@@ -1679,7 +1702,10 @@ int ms_nemesis_grudge(uint32_t seed_lo, uint32_t seed_hi, uint32_t cluster, uint
   std::vector<uint32_t> keys(g);
   for (uint32_t k = 0; k < g; k++) keys[k] = nem_key(seed_lo, seed_hi, op, cluster * g + k);
   const uint32_t m = nem_side_a(target, g);
-  for (uint32_t k = 0; k < g; k++) side_out[k] = nem_rank(keys.data(), g, k) < m ? 0u : 1u;
+  for (uint32_t k = 0; k < g; k++) {
+    const uint32_t r = nem_rank(keys.data(), g, k);
+    side_out[k] = ring ? r : (r < m ? 0u : 1u);
+  }
   return MS_OK;
 }
 

@@ -811,8 +811,30 @@ __global__ void k_wake(Params p) {
 // ------------------------------------------------------------------ k_nemesis (ms_set_nemesis, DESIGN.md 2.13)
 // One CTA before every executed round while the nemesis is on: returns at once unless `now` has reached the
 // earliest pending instant; otherwise performs every due op of every cluster, in (cluster, op) order -- the
-// component ids of the cluster's servers in p.comp and one history record per op -- and recomputes that instant.
+// component ids of the cluster's servers in p.comp (or, for majorities-ring, the cluster's block of the pair matrix)
+// and one history record per op -- and recomputes that instant.
 constexpr int kNemThreads = 512;
+
+// A majorities-ring grudge in the cluster's g x g block of the [dest][src] pair matrix: bit (base + r, base + q) set
+// iff the server at ring position pos[r] does not hear the one at pos[q] (nem_ring_hears); cut = false clears the
+// block.  One item per (row, word); when base or g is not a multiple of 32, a row's first and last words also hold
+// columns of the neighbouring clusters, and the new bits are merged under this cluster's column mask.  Only
+// k_nemesis's one CTA writes the matrix between rounds, and it applies ops one at a time with a barrier in between,
+// so this read-modify-write races with nothing.
+__device__ void nem_ring_block(const Params& p, const uint32_t* pos, uint32_t base, uint32_t g, bool cut) {
+  const uint32_t w0 = base >> 5, words = ((base + g - 1) >> 5) - w0 + 1;
+  for (uint32_t i = threadIdx.x; i < g * words; i += blockDim.x) {
+    const uint32_t r = i / words, w = w0 + i % words;
+    const uint32_t lo = max(base, w * 32u), hi = min(base + g, w * 32u + 32u);   // this word's columns of the block
+    uint32_t mask = 0, bits = 0;
+    for (uint32_t col = lo; col < hi; col++) {
+      mask |= 1u << (col & 31u);
+      if (cut && !nem_ring_hears(pos[r], pos[col - base], g)) bits |= 1u << (col & 31u);
+    }
+    uint32_t* at = p.pair_bits + (size_t)(base + r) * p.pair_words + w;
+    *at = mask == 0xFFFFFFFFu ? bits : (*at & ~mask) | bits;
+  }
+}
 __global__ void __launch_bounds__(kNemThreads) k_nemesis(Params p) {
   __shared__ uint32_t s_key[kNemMaxGroup];
   __shared__ uint32_t s_due[kNemThreads];
@@ -860,11 +882,28 @@ __global__ void __launch_bounds__(kNemThreads) k_nemesis(Params p) {
         const uint32_t act = s_act;
         if (act == 0) break;
         const uint32_t op = s_nd.op, base = c * g;
-        if (act != MS_HF_NEM_STOP) {
+        if (act == MS_HF_NEM_MAJORITIES_RING) {
+          for (uint32_t k = tid; k < g; k += kNemThreads) s_key[k] = nem_key(p.seed_lo, p.seed_hi, op, base + k);
+          __syncthreads();
+          // ring positions: ranked in registers (launched with kNemThreads threads: at most g / kNemThreads each),
+          // then written over the keys once every thread has read them
+          uint32_t pos[kNemMaxGroup / kNemThreads];
+#pragma unroll
+          for (uint32_t j = 0; j < kNemMaxGroup / kNemThreads; j++)
+            if (tid + j * kNemThreads < g) pos[j] = nem_rank(s_key, g, tid + j * kNemThreads);
+          __syncthreads();
+#pragma unroll
+          for (uint32_t j = 0; j < kNemMaxGroup / kNemThreads; j++)
+            if (tid + j * kNemThreads < g) s_key[tid + j * kNemThreads] = pos[j];
+          __syncthreads();
+          nem_ring_block(p, s_key, base, g, true);
+        } else if (act != MS_HF_NEM_STOP) {
           for (uint32_t k = tid; k < g; k += blockDim.x) s_key[k] = nem_key(p.seed_lo, p.seed_hi, op, base + k);
           __syncthreads();
           const uint32_t m = nem_side_a(act, g);
           for (uint32_t k = tid; k < g; k += blockDim.x) p.comp[base + k] = nem_rank(s_key, g, k) < m ? 2u * c : 2u * c + 1u;
+        } else if (s_nd.part == MS_HF_NEM_MAJORITIES_RING) {
+          nem_ring_block(p, s_key, base, g, false);
         } else {
           for (uint32_t k = tid; k < g; k += blockDim.x) p.comp[base + k] = 0xFFFFFFFFu;
         }
@@ -879,7 +918,7 @@ __global__ void __launch_bounds__(kNemThreads) k_nemesis(Params p) {
             at[0] = make_uint4((uint32_t)now, (uint32_t)((uint64_t)now >> 32), (uint32_t)order, (uint32_t)(order >> 32));
             at[1] = make_uint4(MS_H_NEMESIS, op, (uint32_t)MS_H_INFO | (act << 8), c);
           }
-          s_nd.part = act != MS_HF_NEM_STOP;
+          s_nd.part = act != MS_HF_NEM_STOP ? act : 0u;
           s_nd.op = op + 1;
           if (s_nd.t < p.nem_limit_ns) {
             uint32_t x[4];

@@ -15,7 +15,8 @@ constexpr uint32_t kNemMaxGroup = 8192;
 constexpr int64_t  kNemDefaultIntervalNs = 10000000000ll;   // --nemesis-interval 10 (core.clj:206-217)
 constexpr int64_t  kNemMaxIntervalNs = 1ll << 50;           // keeps t_j + 2 interval far from overflow
 
-// Per-cluster state in HBM: the instant of the next op (t_j), its index j, whether the last op was a start.
+// Per-cluster state in HBM: the instant of the next op (t_j), its index j, and the MS_HF_NEM_* code of the start
+// that holds (0 = healthy): a stop clears what that start wrote, `comp` entries or the block of the pair matrix.
 struct NemDev {
   int64_t  t;
   uint32_t op, part;
@@ -38,17 +39,32 @@ MS_HD int64_t nem_pending(const NemDev& n, int64_t limit_ns) {
   return n.t < limit_ns ? n.t : (n.part ? limit_ns : INT64_MAX);
 }
 
-// target mask (0 = all three) and word 1 of the draw -> MS_HF_NEM_ONE / _MAJORITY / _MINORITY_THIRD
+// ms_nemesis_config.targets: bits 0-2 the component targets, bit 3 primaries (refused: the Maelstrom db has none),
+// bit 4 majorities-ring; 0 = the three component targets
+constexpr uint32_t kNemComponentTargets = 7u;
+constexpr uint32_t kNemRingTarget = 0x10u;
+constexpr uint32_t kNemTargetBits = kNemComponentTargets | kNemRingTarget;
+
+// target mask and word 1 of the draw -> MS_HF_NEM_ONE / _MAJORITY / _MINORITY_THIRD / _MAJORITIES_RING: the enabled
+// target (x1 * n_enabled) >> 32 in that order
 MS_HD uint32_t nem_target(uint32_t mask, uint32_t x1) {
-  mask = mask ? (mask & 7u) : 7u;
-  const uint32_t n = (mask & 1u) + ((mask >> 1) & 1u) + ((mask >> 2) & 1u);
+  mask = mask ? (mask & kNemTargetBits) : kNemComponentTargets;
+  const uint32_t n = (mask & 1u) + ((mask >> 1) & 1u) + ((mask >> 2) & 1u) + ((mask >> 4) & 1u);
   uint32_t k = (uint32_t)(((uint64_t)x1 * n) >> 32);
-  for (uint32_t t = 0; t < 3; t++)
+  for (uint32_t t = 0; t < 5; t++)
     if ((mask >> t) & 1u) {
-      if (k == 0) return MS_HF_NEM_ONE + t;
+      if (k == 0) return t == 4 ? (uint32_t)MS_HF_NEM_MAJORITIES_RING : MS_HF_NEM_ONE + t;
       k--;
     }
   return MS_HF_NEM_ONE;
+}
+
+// majorities-ring: the server at ring position p receives from the one at position q iff (q - p + h) mod g < m, with
+// m = g/2 + 1 and h = m/2 -- the window of m consecutive positions starting at i, given to the node at i + h.  Every
+// member hears m members (itself included), no two the same set for g >= 3; the cut is one-way when m is even
+MS_HD bool nem_ring_hears(uint32_t p, uint32_t q, uint32_t g) {
+  const uint32_t m = g / 2 + 1, h = m / 2;
+  return (q + g - p + h) % g < m;
 }
 
 // servers on side A: ranks below this

@@ -242,9 +242,10 @@ class Sim:
 
     def nemesis(self, time_limit_ns, interval_ns=0, start_ns=None, targets=0, group=0):
         """ms_set_nemesis: a Jepsen partition schedule per cluster, run on the device before every round (DESIGN.md
-        2.13).  targets: a mask of NEM_ONE / NEM_MAJORITY / NEM_MINORITY_THIRD (0 = all three); interval_ns 0 = 10 s;
-        start_ns None = now (an earlier instant is refused); group 0 = the workload's clusters.  Each op is a
-        history() record with client H_NEMESIS"""
+        2.13).  targets: a mask of NEM_ONE / NEM_MAJORITY / NEM_MINORITY_THIRD / NEM_MAJORITIES_RING (0 = the first
+        three); interval_ns 0 = 10 s; start_ns None = now (an earlier instant is refused); group 0 = the workload's
+        clusters.  Each op is a history() record with client H_NEMESIS.  With NEM_MAJORITIES_RING the nemesis owns the
+        pairwise matrix: max_endpoints <= 65536, no drop() installed before, drop() refused while it is on"""
         nc = _lib.NemesisConfig(group, targets, interval_ns, self.now if start_ns is None else start_ns, time_limit_ns)
         return self._chk(self.L.ms_set_nemesis(self.h, C.byref(nc)))
 
@@ -422,13 +423,17 @@ HIST_TYPES = ("invoke", "ok", "fail", "info")              # MS_H_*
 HF_KV_READ, HF_KV_WRITE, HF_KV_CAS = 2, 3, 4              # MS_HF_KV_*
 H_NEMESIS = 0xFFFFFFFF                                    # MS_H_NEMESIS: the client of a nemesis record
 HF_NEM_ONE, HF_NEM_MAJORITY, HF_NEM_MINORITY_THIRD, HF_NEM_STOP = 5, 6, 7, 8   # MS_HF_NEM_*
+HF_NEM_MAJORITIES_RING = 9                                # MS_HF_NEM_MAJORITIES_RING
 NEM_ONE, NEM_MAJORITY, NEM_MINORITY_THIRD = 1, 2, 4       # ms_nemesis_config.targets bits
+NEM_MAJORITIES_RING = 16
 
 
 def nemesis_grudge(seed, cluster, g, op, target):
-    """ms_nemesis_grudge: the sides of a nemesis start record (op = its op, target = its f, cluster = its value) in a
-    simulation with this seed and g servers per cluster; uint32 array, entry i = 0 (side A) / 1 (side B) for server
-    cluster * g + i"""
+    """ms_nemesis_grudge: the grudge of a nemesis start record (op = its op, target = its f, cluster = its value) in a
+    simulation with this seed and g servers per cluster; uint32 array, entry i for server cluster * g + i.  For
+    HF_NEM_ONE / _MAJORITY / _MINORITY_THIRD it is 0 (side A) / 1 (side B); for HF_NEM_MAJORITIES_RING it is the
+    server's ring position p, and the server at p receives from the one at q iff (q - p + h) % g < m, with
+    m = g // 2 + 1 and h = m // 2"""
     out = np.zeros(max(g, 1), dtype=np.uint32)
     rc = _lib.lib().ms_nemesis_grudge(seed & 0xFFFFFFFF, seed >> 32, cluster, g, op, target, out.ctypes.data)
     if rc < 0:
