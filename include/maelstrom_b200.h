@@ -167,7 +167,8 @@ typedef struct ms_config {
   uint32_t mailbox_cap;      /* host-visible deliveries buffered between syncs */
   uint32_t inject_cap;       /* host sends staged per round */
   int32_t  device;           /* CUDA device ordinal */
-  uint32_t threads_per_node; /* CTA size of the round kernel (0 = auto) */
+  uint32_t threads_per_node; /* CTA size of the round kernel (0 = auto); a multiple of 32 in [32, 512], at most 256
+                              * in the size classes of windows up to 2048 */
   uint32_t n_shards;         /* GPUs the endpoints are sharded over (0/1 = single GPU), <= 8 */
   uint32_t shard_id;         /* this process's shard */
   uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn node (0 = 4096) */

@@ -641,7 +641,7 @@ static int build_sim(ms_sim* s, const ms_config* in) {
   if (c.n_shards == 0) c.n_shards = 1;
   if (c.n_shards > 8 || c.shard_id >= c.n_shards) { set_err("n_shards must be <= 8 and shard_id < n_shards"); return MS_ERR_ARG; }
   if (c.threads_per_node && (c.threads_per_node % 32 || c.threads_per_node > 512)) {
-    set_err("threads_per_node must be a multiple of 32 in [32,512]");
+    set_err("threads_per_node must be a multiple of 32 in [32,512] (above 256 it widens only the class of windows > 2048)");
     return MS_ERR_ARG;
   }
   {
@@ -653,7 +653,10 @@ static int build_sim(ms_sim* s, const ms_config* in) {
     for (int k = 0; k < 4; k++) {
       const uint32_t cap = std::min(ladder[k], c.max_window);
       s->class_cap[s->n_classes] = cap;
-      s->class_threads[s->n_classes] = c.threads_per_node ? (int)c.threads_per_node : thr[k];
+      // k_round of classes 0-2 is compiled for at most 256 threads per CTA (its launch bounds), class 3 for 512:
+      // a wider threads_per_node applies to class 3 only
+      const int max_thr = k < 3 ? 256 : 512;
+      s->class_threads[s->n_classes] = c.threads_per_node ? std::min((int)c.threads_per_node, max_thr) : thr[k];
       s->n_classes++;
       if (cap == c.max_window) break;
     }
