@@ -116,8 +116,18 @@ enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* 
                              ms_config.reserved[3] = pointers a node may mint (default 256), reserved[4] = tree nodes a node
                              may cache (default 1024), reserved[2] (service keys) defaults to cover every pointer.
                              A sync RPC without a reply times out after 5 s (promise.rb): error 0 to the client. */
-       MS_W_TXN = 4 };   /* txn-list-append, whole database in one lin-kv key (demo/clojure/single_key_txn.clj);
+       MS_W_TXN = 4,     /* txn-list-append, whole database in one lin-kv key (demo/clojure/single_key_txn.clj);
                             needs the "lin-kv" service endpoint */
+       MS_W_KV_PROXY = 6 };/* lin-kv served by proxies of a kv service (demo/ruby/lin_kv_proxy.rb, DESIGN.md 2.14): a node
+                            forwards read / write / cas to the service ms_config.reserved[3] names (MS_SVC_LIN_KV, the
+                            default, MS_SVC_SEQ_KV or MS_SVC_LWW_KV; anything else is MS_ERR_ARG) with msg_id = its
+                            next id from 1 and MS_F_CREATE kept, and answers the client with the service's reply
+                            (type, p0, p1, flags but MS_F_MSG_ID) in_reply_to the client's msg_id -- none when the
+                            request had none.  init -> init_ok, every time.  Replies without a live closure are
+                            ignored; reserved[5] closure slots (a reply after that many newer RPCs is dropped).  Any
+                            other request type crashes the node: later messages are received, with no effect, and it
+                            never sends again.  A missing service endpoint latches "Invalid dest".  No timers; one GPU.
+                            reserved[4] = g groups the servers for ms_add_kv_clients only. */
 enum { MS_TOPO_GRID = 0, MS_TOPO_LINE = 1, MS_TOPO_TOTAL = 2,                /* --topology, broadcast.clj:169-178 */
        MS_TOPO_TREE2 = 3, MS_TOPO_TREE3 = 4, MS_TOPO_TREE4 = 5 };
 enum { MS_DIST_CONSTANT = 0, MS_DIST_UNIFORM = 1, MS_DIST_EXPONENTIAL = 2 }; /* --latency-dist, net.clj:73-77 */
@@ -171,7 +181,7 @@ typedef struct ms_config {
                               * in the size classes of windows up to 2048 */
   uint32_t n_shards;         /* GPUs the endpoints are sharded over (0/1 = single GPU), <= 8 */
   uint32_t shard_id;         /* this process's shard */
-  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn node (0 = 4096) */
+  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn / proxy node (0 = 4096).  MS_W_KV_PROXY: [3] = the backing service MS_SVC_*, [4] = g for ms_add_kv_clients */
   /* ABI 2.  Servers and the other endpoints (clients, hosts, services) may be sized apart: a
    * service hears from every node, a node from a few.  0 = ring_cap / max_window. */
   uint32_t server_ring_cap;  /* inbox ring capacity of the servers, power of two */
@@ -290,7 +300,9 @@ typedef struct ms_kv_gen_config {
   int64_t  key_period_ns;    /* > 0: virtual time a group spends on one key */
 } ms_kv_gen_config;
 enum { MS_HF_KV_READ = 2, MS_HF_KV_WRITE = 3, MS_HF_KV_CAS = 4 };
-/* adds cfg->n_clients endpoints "c<first_name> ..." and returns the index of the first.  MS_W_RAFT on one GPU,
+/* adds cfg->n_clients endpoints "c<first_name> ..." and returns the index of the first.  MS_W_RAFT or MS_W_KV_PROXY
+ * (the same rules, g = ms_config.reserved[4], except that the proxies share one store, the service's: key_base =
+ * group * keys_per_group, so every group has its own keys; a proxy passes on the service's errors 20 and 22, :fail) on one GPU,
  * once per simulation, not together with ms_add_gen_clients; the history comes out of ms_history_drain */
 int ms_add_kv_clients(ms_sim* sim, const ms_kv_gen_config* cfg, uint32_t first_name);
 
@@ -455,7 +467,8 @@ uint64_t ms_client_replies(ms_sim* sim);
 uint64_t ms_undeliverable(ms_sim* sim);
 /* MS_W_RAFT: out = {state (0 nascent, 1 follower, 2 candidate, 3 leader), current_term,
  * voted_for + 1, commit_index, last_applied, leader + 1, log size, keys in the KV store}
- * (the fields of RaftNode, demo/python/raft.py:196-221) */
+ * (the fields of RaftNode, demo/python/raft.py:196-221).
+ * MS_W_KV_PROXY: out = {crashed (0 / 1), the last msg_id sent (@next_msg_id), closures pending, 0, 0, 0, 0, 0} */
 int      ms_raft_state(ms_sim* sim, uint32_t node, uint64_t out[8]);
 
 /* device-side counters for roofline accounting: out = {rounds, sends, recvs,

@@ -254,6 +254,8 @@ struct Params {
   struct NemDev* nem;
   uint32_t  nem_clusters, nem_group, nem_targets, nem_pad;
   int64_t   nem_interval_ns, nem_limit_ns;
+  // MS_W_KV_PROXY (kp_handle in csrc/ms_raft.cuh): the backing service, MS_SVC_*.  Appended
+  uint32_t  kp_service, kp_pad;
 };
 
 constexpr uint32_t kRaftCallbacks = 4096;       // default pending-RPC table slots per node (ms_config.reserved[5]; oracle: same)

@@ -511,7 +511,8 @@ struct ms_sim {
     if (b.flags & MS_F_MSG_ID) kv.push_back({"msg_id", false, (int64_t)b.msg_id, ""});
     if (b.flags & MS_F_REPLY) kv.push_back({"in_reply_to", false, (int64_t)b.in_reply_to, ""});
     const bool kv_peer = (e.src < kinds.size() && (kinds[e.src] & 0x7F) == MS_KIND_SERVICE) ||
-                         (e.dest < kinds.size() && (kinds[e.dest] & 0x7F) == MS_KIND_SERVICE) || cfg.workload == MS_W_RAFT;
+                         (e.dest < kinds.size() && (kinds[e.dest] & 0x7F) == MS_KIND_SERVICE) || cfg.workload == MS_W_RAFT ||
+                         cfg.workload == MS_W_KV_PROXY;
     const int64_t lo = (int64_t)(b.p1 & 0xFFFFFFFFull), hi = (int64_t)(b.p1 >> 32);
     switch (b.type) {
       case MS_T_BROADCAST: kv.push_back({"message", false, (int64_t)b.p0, ""}); break;
@@ -598,7 +599,7 @@ static int build_sim(ms_sim* s, const ms_config* in) {
   ms_config& c = s->cfg;
   c = *in;
   if (c.n_nodes == 0) { set_err("n_nodes must be positive (--node-count)"); return MS_ERR_ARG; }
-  if (c.workload > MS_W_TXN_TREE || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
+  if (c.workload > MS_W_KV_PROXY || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
     set_err("bad workload/topology/latency_dist");
     return MS_ERR_ARG;
   }
@@ -784,9 +785,21 @@ static int build_sim(ms_sim* s, const ms_config* in) {
     CK(cudaMemcpyAsync(P.tt_recs + (size_t)(mst::kPtrEmpty - 1u) * 64, &empty, sizeof empty, cudaMemcpyHostToDevice, s->stream));
     CK(cudaStreamSynchronize(s->stream));
   }
-  if (c.workload == MS_W_TXN || c.workload == MS_W_TXN_TREE) {
-    // txn-list-append nodes: message ids, the table of pending RPC closures and the staging rows of
-    // the sequential step (csrc/ms_raft.cuh)
+  if (c.workload == MS_W_KV_PROXY) {
+    // lin-kv proxies (kp_handle, csrc/ms_raft.cuh): reserved[3] names the backing service, reserved[4] = g only binds
+    // the kv clients (ms_add_kv_clients); the nodes keep what the txn nodes keep, below
+    if (c.n_shards > 1) { set_err("MS_W_KV_PROXY runs on one GPU"); return MS_ERR_ARG; }
+    if (c.reserved[3] > MS_SVC_LWW_KV) {
+      set_err("MS_W_KV_PROXY: ms_config.reserved[3] must name lin-kv, seq-kv or lww-kv (MS_SVC_LIN_KV / _SEQ_KV / _LWW_KV)");
+      return MS_ERR_ARG;
+    }
+    P.kp_service = c.reserved[3];
+    P.rf_n_keys = c.reserved[2] ? c.reserved[2] : 4096u;           // the service's keys bound the clients' key ranges
+    P.rf_group = (c.reserved[4] && c.reserved[4] < c.n_nodes) ? c.reserved[4] : 0u;
+  }
+  if (c.workload == MS_W_TXN || c.workload == MS_W_TXN_TREE || c.workload == MS_W_KV_PROXY) {
+    // txn-list-append nodes and lin-kv proxies: message ids, the table of pending RPC closures and the staging rows
+    // of the sequential step (csrc/ms_raft.cuh); a proxy sends at most once per message it receives
     // (nothing here is read across nodes: sharded runs need no extra mapping)
     const size_t N = c.n_nodes;
     P.rf_stage_cap = c.workload == MS_W_TXN_TREE ? c.server_max_window * (mst::kMaxWrites + 2u) + 64u : c.server_max_window + 16u;
@@ -1130,7 +1143,10 @@ int ms_add_kv_clients(ms_sim* s, const ms_kv_gen_config* kc, uint32_t first_name
     set_err("ms_add_kv_clients: bad configuration");
     return MS_ERR_ARG;
   }
-  if (s->cfg.workload != MS_W_RAFT) { set_err("ms_add_kv_clients: the lin-kv clients drive the Raft nodes (MS_W_RAFT)"); return MS_ERR_ARG; }
+  if (s->cfg.workload != MS_W_RAFT && s->cfg.workload != MS_W_KV_PROXY) {
+    set_err("ms_add_kv_clients: the lin-kv clients drive the Raft nodes (MS_W_RAFT) or the lin-kv proxies (MS_W_KV_PROXY)");
+    return MS_ERR_ARG;
+  }
   if (s->P.gc) { set_err("ms_add_kv_clients: the generator's clients exist already"); return MS_ERR_ARG; }
   if (s->P.n_shards > 1) { set_err("ms_add_kv_clients: single GPU only"); return MS_ERR_ARG; }
   Params& P = s->P;
@@ -1141,9 +1157,12 @@ int ms_add_kv_clients(ms_sim* s, const ms_kv_gen_config* kc, uint32_t first_name
     return MS_ERR_ARG;
   }
   const uint32_t n_groups = kc->n_clients / (2u * gsz);
-  const uint64_t keys = (uint64_t)((n_groups + n_clusters - 1u) / n_clusters) * kc->keys_per_group;   // per cluster
+  // key ranges are disjoint within one store: a Raft cluster's, or the one service every lin-kv proxy forwards to
+  const uint32_t key_clusters = s->cfg.workload == MS_W_KV_PROXY ? 1u : n_clusters;
+  const uint64_t keys = (uint64_t)((n_groups + key_clusters - 1u) / key_clusters) * kc->keys_per_group;   // per store
   if (keys > std::min<uint64_t>(P.rf_n_keys, 1u << 16)) {
-    set_err("ms_add_kv_clients: the groups of a cluster need " + std::to_string(keys) + " keys, more than ms_config.reserved[2] or 65536");
+    set_err("ms_add_kv_clients: the groups of one store (a Raft cluster, or the service of the lin-kv proxies) need " +
+            std::to_string(keys) + " keys, more than ms_config.reserved[2] or 65536");
     return MS_ERR_ARG;
   }
   if ((uint64_t)P.n_ep + kc->n_clients > s->cfg.max_endpoints) { set_err("max_endpoints exhausted"); return MS_ERR_CAPACITY; }
@@ -1171,7 +1190,7 @@ int ms_add_kv_clients(ms_sim* s, const ms_kv_gen_config* kc, uint32_t first_name
     s->mailbox.emplace_back();
     s->by_name[id] = idx;
     init[k].node = (group % n_clusters) * gsz + k % gsz;
-    init[k].key_base = (group / n_clusters) * kc->keys_per_group;
+    init[k].key_base = (group / key_clusters) * kc->keys_per_group;
     init[k].reader = k % (2u * gsz) < gsz;
     init[k].ordinal = k;
   }
@@ -1495,7 +1514,8 @@ int ms_recv_json(ms_sim* s, uint32_t e, int64_t timeout, char* out, size_t cap) 
   body["type"] = msj::quote(t);
   if (m.flags & MS_F_MSG_ID) body["msg_id"] = std::to_string(m.msg_id);
   if (m.flags & MS_F_REPLY) body["in_reply_to"] = std::to_string(m.in_reply_to);
-  const bool kv_peer = (m.src < s->kinds.size() && (s->kinds[m.src] & 0x7F) == MS_KIND_SERVICE) || s->cfg.workload == MS_W_RAFT;
+  const bool kv_peer = (m.src < s->kinds.size() && (s->kinds[m.src] & 0x7F) == MS_KIND_SERVICE) || s->cfg.workload == MS_W_RAFT ||
+                       s->cfg.workload == MS_W_KV_PROXY;
   const uint32_t lo = (uint32_t)m.p1, hi = (uint32_t)(m.p1 >> 32);
   bool blob_ok = true;
   switch (m.type) {
@@ -2064,6 +2084,11 @@ int ms_raft_state(ms_sim* s, uint32_t node, uint64_t out[8]) {
   RaftDev r;
   CK(cudaStreamSynchronize(s->stream));
   CK(cudaMemcpy(&r, s->P.rf_node + node, sizeof r, cudaMemcpyDeviceToHost));
+  if (s->cfg.workload == MS_W_KV_PROXY) {   // kp_handle's fields: crashed, @next_msg_id, closures pending
+    out[0] = (uint64_t)r.state; out[1] = r.next_msg_id; out[2] = r.kv_size;
+    for (int k = 3; k < 8; k++) out[k] = 0;
+    return MS_OK;
+  }
   out[0] = (uint64_t)r.state; out[1] = r.term; out[2] = (uint64_t)(r.voted_for + 1); out[3] = r.commit_index;
   out[4] = r.last_applied; out[5] = (uint64_t)(r.leader + 1); out[6] = r.log_size; out[7] = r.kv_size;
   return MS_OK;

@@ -1644,6 +1644,7 @@ __device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t
     const uint4* rp = w.ring + (size_t)((w.head + i) & w.mask) * 3;
     if (p.workload == MS_W_RAFT) rf_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else if (p.workload == MS_W_TXN_TREE) tt_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+    else if (p.workload == MS_W_KV_PROXY) kp_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else txn_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
   }
   if (p.workload == MS_W_RAFT) { rf_actions(c); rf_note_busy(c); }

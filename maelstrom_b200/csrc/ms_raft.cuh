@@ -474,6 +474,60 @@ __device__ void txn_handle(RaftCtx& c, const Rec& m) {
   rf_emit(c, er);
 }
 
+// ------------------------------------------------------------------ lin-kv proxy
+// demo/ruby/lin_kv_proxy.rb on node.rb (DESIGN.md 2.14): read / write / cas are forwarded to the backing service
+// (Params.kp_service) by rpc!, and the service's reply, minus its msg_id, goes back to the client by reply!.  Handlers
+// run in dequeue order, a legal schedule of Ruby's thread per message.  Uses RaftDev.state (1 = crashed: main! raised
+// on a message without a handler), .next_msg_id (@next_msg_id) and .kv_size (closures pending).  A closure is
+// {msg_id, 1, the client's msg_id, the client} + {the request had a msg_id}.
+__device__ void kp_answer(RaftCtx& c, uint32_t client, uint32_t client_msg_id, bool had_msg_id, uint32_t type,
+                          uint32_t flags, uint32_t p0, uint64_t p1) {
+  Rec a;                                                                          // reply! (node.rb:88-91)
+  a.round = 0; a.ticket = 0; a.idx = 0;
+  a.src = c.e; a.dest = client; a.msg_id = 0;
+  a.in_reply_to = had_msg_id ? client_msg_id : 0u;                                // in_reply_to: nil without a msg_id
+  flags &= ~(uint32_t)(MS_F_MSG_ID | MS_F_REPLY);
+  a.tf = type | ((flags | (had_msg_id ? (uint32_t)MS_F_REPLY : 0u)) << 16);
+  a.p0 = p0; a.p1 = p1;
+  rf_emit(c, a);
+}
+
+__device__ void kp_handle(RaftCtx& c, const Rec& m) {
+  RaftDev* r = c.r;
+  if (r->state) return;                                                           // crashed: read, never acted on
+  const uint32_t type = m.tf & 0xFFFFu, flags = m.tf >> 16;
+  if (flags & MS_F_REPLY) {                                                       // main!, node.rb:159-164
+    uint4* slot = c.cb + 2 * (size_t)(m.in_reply_to & c.p.rf_cb_mask);
+    const uint4 s0 = slot[0], s1 = slot[1];
+    if (s0.y == 0 || s0.x != m.in_reply_to) return;                               // "Ignoring reply ... with no callback"
+    slot[0] = make_uint4(0u, 0u, 0u, 0u);
+    r->kv_size--;
+    kp_answer(c, s0.w, s0.z, s1.x != 0, type, flags, m.p0, m.p1);                 // proxy!'s block
+    return;
+  }
+  if (type == MS_T_INIT) {                                                        // node.rb:22-36
+    kp_answer(c, m.src, m.msg_id, (flags & MS_F_MSG_ID) != 0, MS_T_INIT_OK, 0u, 0u, 0ull);
+    return;
+  }
+  if (type == MS_T_READ || type == MS_T_WRITE || type == MS_T_CAS) {              // proxy!, lin_kv_proxy.rb:27-38
+    const uint32_t svc = c.p.sv_ep[c.p.kp_service];
+    if (svc == 0xFFFFFFFFu) { latch_error(c.st, E_INVALID_DEST, svc); return; }   // no such service endpoint
+    const uint32_t id = ++r->next_msg_id;                                         // rpc!, node.rb:95-102
+    uint4* slot = c.cb + 2 * (size_t)(id & c.p.rf_cb_mask);
+    if (slot[0].y == 0) r->kv_size++;                                             // else it takes an older closure's slot
+    slot[0] = make_uint4(id, 1u, m.msg_id, m.src);
+    slot[1] = make_uint4((flags & MS_F_MSG_ID) ? 1u : 0u, 0u, 0u, 0u);
+    Rec q;
+    q.round = 0; q.ticket = 0; q.idx = 0;
+    q.src = c.e; q.dest = svc; q.msg_id = id; q.in_reply_to = 0;
+    q.tf = type | ((uint32_t)(MS_F_MSG_ID | (flags & MS_F_CREATE)) << 16);
+    q.p0 = m.p0; q.p1 = m.p1;
+    rf_emit(c, q);
+    return;
+  }
+  r->state = 1;                                                                   // "No handler": main! raises, node.rb:167
+}
+
 // ------------------------------------------------------------------ txn-list-append on a persistent hash tree
 // demo/ruby/datomic_list_append.rb.  The database is a tree of immutable nodes stored in lww-kv under
 // unique pointers; lin-kv holds the pointer to the root (key "root" = key 0 here).  A txn (:340-353, under

@@ -8,7 +8,8 @@ import numpy as np
 from . import _lib
 from ._lib import Body, Config, EVENT_DTYPE, JBODY_DTYPE, MSG_DTYPE, OP_DTYPE  # noqa: F401
 
-WORKLOADS = {"echo": 0, "broadcast": 1, "g-set": 2, "lin-kv": 3, "txn-list-append": 4, "txn-list-append-tree": 5}
+WORKLOADS = {"echo": 0, "broadcast": 1, "g-set": 2, "lin-kv": 3, "txn-list-append": 4, "txn-list-append-tree": 5,
+             "lin-kv-proxy": 6}
 TOPOLOGIES = {"grid": 0, "line": 1, "total": 2, "tree": 3, "tree2": 3, "tree3": 4, "tree4": 5}
 DISTS = {"constant": 0, "uniform": 1, "exponential": 2}
 KIND_SERVER, KIND_CLIENT, KIND_HOST, KIND_SIM_CLIENT, KIND_SERVICE = 0, 1, 2, 3, 4
@@ -88,6 +89,10 @@ class Sim:
         cfg.p_loss = p_loss
         cfg.n_values = n_values
         cfg.journal_level = 2
+        # lin-kv-proxy: the service the proxies forward to (ms_config.reserved[3], MS_SVC_*)
+        if "proxy_service" in sizing:
+            name = sizing.pop("proxy_service")
+            cfg.reserved[3] = SERVICES.index(name) if isinstance(name, str) else int(name)
         # named spellings of ms_config.reserved[]
         for name, slot in (("history_rounds", 0), ("use_graph", 1), ("n_keys", 2), ("raft_log_cap", 3),
                            ("raft_group", 4), ("rpc_table", 5), ("tree_ptrs", 3), ("tree_cache", 4)):
@@ -160,7 +165,7 @@ class Sim:
 
     def add_kv_clients(self, n_clients, interval_ns, time_limit_ns, key_period_ns, keys_per_group=1, value_range=0,
                        timeout_ns=0, first_name=0):
-        """ms_add_kv_clients: closed-loop lin-kv clients of the Raft nodes on the device (groups of 2g per key,
+        """ms_add_kv_clients: closed-loop lin-kv clients of the Raft nodes or the lin-kv proxies on the device (groups of 2g per key,
         half of them readers); returns the first endpoint index.  history() returns their records,
         kv_history(records, *sim.kv_groups) sorts them into one history per register"""
         kc = _lib.KvGenConfig(n_clients, value_range, keys_per_group, interval_ns, timeout_ns, time_limit_ns,
@@ -417,6 +422,15 @@ class Sim:
         d["voted_for"] -= 1
         d["leader"] -= 1
         return d
+
+    PROXY_FIELDS = ("crashed", "next_msg_id", "pending")
+
+    def proxy_state(self, node):
+        """a lin-kv proxy's fields (ms_raft_state on MS_W_KV_PROXY): crashed 0 / 1, the last msg_id it sent, closures
+        pending"""
+        out = np.zeros(8, dtype=np.uint64)
+        self._chk(self.L.ms_raft_state(self.h, node, out.ctypes.data))
+        return dict(zip(self.PROXY_FIELDS, (int(x) for x in out[:3])))
 
 
 HIST_TYPES = ("invoke", "ok", "fail", "info")              # MS_H_*
