@@ -103,7 +103,14 @@ enum {
    * contains an append; txn_ok p1 = version read | version written << 32.  Database values are
    * carried as version ids: 0 = nil (no root yet), 1 = the empty database, others minted by the
    * node whose cas installs them; the caller replays apply-txn (single_key_txn.clj:115-127) over them */
-  MS_T_TXN = 60, MS_T_TXN_OK = 61
+  MS_T_TXN = 60, MS_T_TXN_OK = 61,
+  /* kafka (workload/kafka.clj:88-150, DESIGN.md 2.15).  Keys < 65535, 0xFFFF = no key; offsets 32-bit.
+   * send p0 = key, p1 = msg; send_ok p1 = offset.  poll / commit_offsets p0 = k0 | k1 << 16, p1 = o0 | o1 << 32;
+   * poll_ok p0 = the keys that have messages (0xFFFF for the others), p1 = len0 | len1 << 32: the log of key i
+   * has len_i messages and [o_i, len_i) is what the poll returns (ms_kafka_log).  commit_offsets_ok: empty.
+   * list_committed_offsets p0 = k0 | k1 << 16; its _ok p0 = the keys that are present, p1 = their offsets. */
+  MS_T_SEND = 70, MS_T_SEND_OK = 71, MS_T_POLL = 72, MS_T_POLL_OK = 73, MS_T_COMMIT_OFFSETS = 74,
+  MS_T_COMMIT_OFFSETS_OK = 75, MS_T_LIST_COMMITTED_OFFSETS = 76, MS_T_LIST_COMMITTED_OFFSETS_OK = 77
 };
 
 enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* --workload, core.clj:36-47 */
@@ -118,7 +125,7 @@ enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* 
                              A sync RPC without a reply times out after 5 s (promise.rb): error 0 to the client. */
        MS_W_TXN = 4,     /* txn-list-append, whole database in one lin-kv key (demo/clojure/single_key_txn.clj);
                             needs the "lin-kv" service endpoint */
-       MS_W_KV_PROXY = 6 };/* lin-kv served by proxies of a kv service (demo/ruby/lin_kv_proxy.rb, DESIGN.md 2.14): a node
+       MS_W_KV_PROXY = 6,  /* lin-kv served by proxies of a kv service (demo/ruby/lin_kv_proxy.rb, DESIGN.md 2.14): a node
                             forwards read / write / cas to the service ms_config.reserved[3] names (MS_SVC_LIN_KV, the
                             default, MS_SVC_SEQ_KV or MS_SVC_LWW_KV; anything else is MS_ERR_ARG) with msg_id = its
                             next id from 1 and MS_F_CREATE kept, and answers the client with the service's reply
@@ -128,6 +135,15 @@ enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* 
                             other request type crashes the node: later messages are received, with no effect, and it
                             never sends again.  A missing service endpoint latches "Invalid dest".  No timers; one GPU.
                             reserved[4] = g groups the servers for ms_add_kv_clients only. */
+       MS_W_KAFKA = 7 };   /* kafka served by single-node logs (demo/clojure/kafka_single_node.clj, DESIGN.md 2.15): every
+                            node keeps its own append-only log per key, ms_config.reserved[2] keys (0 = 16, <= 65535) of
+                            reserved[3] messages each (0 = 4096).  init -> init_ok; send appends and answers offset =
+                            count - 1; poll answers every requested key whose log is longer than the offset;
+                            commit_offsets merges with max; list_committed_offsets selects the committed keys.  A
+                            message with in_reply_to is ignored; any other type gets error 10 and the node goes on.
+                            A key >= reserved[2] latches E_VALUE_RANGE, an append to a full log a capacity error
+                            (MS_ERR_SIM).  reserved[4] = g groups the servers for ms_add_kafka_clients (0 = 1).  No
+                            timers; one GPU. */
 enum { MS_TOPO_GRID = 0, MS_TOPO_LINE = 1, MS_TOPO_TOTAL = 2,                /* --topology, broadcast.clj:169-178 */
        MS_TOPO_TREE2 = 3, MS_TOPO_TREE3 = 4, MS_TOPO_TREE4 = 5 };
 enum { MS_DIST_CONSTANT = 0, MS_DIST_UNIFORM = 1, MS_DIST_EXPONENTIAL = 2 }; /* --latency-dist, net.clj:73-77 */
@@ -181,7 +197,7 @@ typedef struct ms_config {
                               * in the size classes of windows up to 2048 */
   uint32_t n_shards;         /* GPUs the endpoints are sharded over (0/1 = single GPU), <= 8 */
   uint32_t shard_id;         /* this process's shard */
-  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn / proxy node (0 = 4096).  MS_W_KV_PROXY: [3] = the backing service MS_SVC_*, [4] = g for ms_add_kv_clients */
+  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn / proxy node (0 = 4096).  MS_W_KV_PROXY: [3] = the backing service MS_SVC_*, [4] = g for ms_add_kv_clients.  MS_W_KAFKA: [2] = keys per node (0 = 16, <= 65535), [3] = log capacity per key (0 = 4096), [4] = g for ms_add_kafka_clients (0 = 1) */
   /* ABI 2.  Servers and the other endpoints (clients, hosts, services) may be sized apart: a
    * service hears from every node, a node from a few.  0 = ring_cap / max_window. */
   uint32_t server_ring_cap;  /* inbox ring capacity of the servers, power of two */
@@ -305,6 +321,63 @@ enum { MS_HF_KV_READ = 2, MS_HF_KV_WRITE = 3, MS_HF_KV_CAS = 4 };
  * group * keys_per_group, so every group has its own keys; a proxy passes on the service's errors 20 and 22, :fail) on one GPU,
  * once per simulation, not together with ms_add_gen_clients; the history comes out of ms_history_drain */
 int ms_add_kv_clients(ms_sim* sim, const ms_kv_gen_config* cfg, uint32_t first_name);
+
+/* Closed-loop kafka clients on the device (MS_W_KAFKA, DESIGN.md 2.15): the Client of workload/kafka.clj:191-241
+ * with the generator below (jepsen.tests.kafka's is not in the reference).  The client side is that of
+ * ms_add_kv_clients: one outstanding request, msg_id from 1, only in_reply_to is matched, timeout_ns per request,
+ * stagger uniform on [0, 2 interval) from the client's own Philox stream (op, endpoint, 0xC11E47, 0).
+ *   binding  n_clients is a multiple of n_nodes; client k talks to server k mod n_nodes, its group is
+ *            (k mod n_nodes) / g (g = ms_config.reserved[4], 0 = 1).  Every client works on keys [0, K),
+ *            K = reserved[2], so the clients of a group share their keys
+ *   ops      r = (word 0 * 1000) >> 32: r < assign_permille assign, then crash_permille crash, else word 3 bit 0
+ *            picks send (0) or poll (1).  assign: k0 = (word 2 * K) >> 32, and with K >= 2 and word 3 bit 0 set a
+ *            second key k1 = (k0 + 1 + ((word 3 * (K - 1)) >> 32)) mod K; then list_committed_offsets, and the
+ *            local offset of a key is kept if it was assigned, else the committed one, else 0 (:204-219).
+ *            crash: :info at once.  send: key (word 2 * K) >> 32, msg = k + n_clients * j for the client's j-th
+ *            send.  poll: the assigned keys at their local offsets; offsets advance to the length returned; a
+ *            poll with messages is followed by commit_offsets of the highest offset polled per key, and the op
+ *            completes with its commit_offsets_ok (:156-164, :223-231)
+ *   reopen   every :info (a crash, a send or poll timing out or an indefinite error) reopens the client: its
+ *            assignment and offsets are cleared; the msg_id counter goes on, so stale replies are discarded
+ *   outcome  with-errors #{:assign} (:202): an assign that times out is :fail, a send or poll :info; definite
+ *            error codes :fail
+ *   end      nothing is invoked at or after time_limit_ns; an op outstanding then still completes or times out
+ *   history  ms_kafka_hist records in ms_kafka_history_drain (ms_history_drain keeps only a nemesis's records) */
+typedef struct ms_kafka_gen_config {
+  uint32_t n_clients;        /* a multiple of n_nodes */
+  uint32_t assign_permille;  /* share of assign ops, out of 1000 */
+  uint32_t crash_permille;   /* share of crash ops; assign_permille + crash_permille <= 1000 */
+  uint32_t pad;
+  int64_t  interval_ns;      /* mean delay between two ops of one client */
+  int64_t  timeout_ns;       /* 0 = 5 000 ms (client.clj:18-20) */
+  int64_t  time_limit_ns;    /* --time-limit */
+} ms_kafka_gen_config;
+typedef struct ms_kafka_hist {
+  int64_t  time_ns;
+  uint64_t order;            /* round << 24 | client ordinal, as ms_hist */
+  uint32_t client;           /* endpoint index */
+  uint32_t op;               /* the client's op counter: an invocation and its completion share it */
+  uint8_t  type;             /* MS_H_INVOKE / OK / FAIL / INFO */
+  uint8_t  f;                /* MS_HF_KAFKA_* */
+  uint16_t error;            /* completion by an error reply: its code; MS_H_TIMEOUT for :net-timeout */
+  /* up to two slots (key, a, b), key 0xFFFF = none.  send: (key, msg, offset; 0xFFFFFFFF before send_ok).  poll
+   * invoke: (key, offset, 0); poll ok: (key, first offset, length) for the keys with messages -- the messages are
+   * ms_kafka_log(node, key)[first, length).  assign invoke: (key, 0, 0); assign ok: (key, start offset, committed
+   * offset or 0xFFFFFFFF).  A :fail or :info completion repeats its invocation's slots, but for a poll that
+   * failed in its commit_offsets, which carries the poll's ok slots */
+  uint32_t key[2], a[2], b[2];
+  uint32_t pad[3];
+} ms_kafka_hist;
+enum { MS_HF_KAFKA_SEND = 10, MS_HF_KAFKA_POLL = 11, MS_HF_KAFKA_ASSIGN = 12, MS_HF_KAFKA_CRASH = 13 };
+/* adds cfg->n_clients endpoints "c<first_name> ..." and returns the index of the first.  MS_W_KAFKA on one GPU, once
+ * per simulation, not together with the other closed-loop clients */
+int ms_add_kafka_clients(ms_sim* sim, const ms_kafka_gen_config* cfg, uint32_t first_name);
+/* The kafka clients' records in (time, round, client) order, as ms_history_drain */
+int ms_kafka_history_drain(ms_sim* sim, ms_kafka_hist* out, size_t cap, size_t* n_out);
+/* MS_W_KAFKA: the messages of node's log of `key` (offset order; at most cap copied) and *len = its length */
+int ms_kafka_log(ms_sim* sim, uint32_t node, uint32_t key, uint32_t* msgs, size_t cap, size_t* len);
+/* MS_W_KAFKA: node's committed offset of `key`, -1 when none; MS_ERR_ARG on another workload or a bad node / key */
+int64_t ms_kafka_committed(ms_sim* sim, uint32_t node, uint32_t key);
 
 /* Upload a time-sorted schedule of client ops (appends). */
 int ms_schedule_ops(ms_sim* sim, const ms_op* ops, size_t n);

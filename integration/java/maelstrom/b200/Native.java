@@ -27,6 +27,8 @@ public final class Native {
   public static native int addGenClients(long h, ByteBuffer msGenConfig, int firstName);
   public static native int addKvClients(long h, ByteBuffer msKvGenConfig, int firstName);
   public static native long historyDrain(long h, ByteBuffer msHist32, long cap);
+  public static native int addKafkaClients(long h, ByteBuffer msKafkaGenConfig, int firstName);
+  public static native long kafkaHistoryDrain(long h, ByteBuffer msKafkaHist64, long cap);
   public static native int scheduleOps(long h, ByteBuffer msOps, long n);
   public static native int step(long h, long nRounds);
   public static native int run(long h, long untilNs);
@@ -58,6 +60,8 @@ public final class Native {
   public static native long clientReplies(long h);
   public static native long undeliverable(long h);
   public static native int raftState(long h, int node, ByteBuffer out8);
+  public static native long kafkaLog(long h, int node, int key, ByteBuffer msgsU32, long cap);
+  public static native long kafkaCommitted(long h, int node, int key);
   public static native int counters(long h, ByteBuffer out8);
   public static native int ringCounters(long h, ByteBuffer out, int n);
   public static native int setOrigin(long h, long round, long msgId, long eventId, int ringPos, int ringStride);

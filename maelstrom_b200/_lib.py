@@ -55,6 +55,11 @@ class KvGenConfig(C.Structure):   # ms_kv_gen_config
                 ("key_period_ns", C.c_int64)]
 
 
+class KafkaGenConfig(C.Structure):   # ms_kafka_gen_config
+    _fields_ = [("n_clients", C.c_uint32), ("assign_permille", C.c_uint32), ("crash_permille", C.c_uint32),
+                ("pad", C.c_uint32), ("interval_ns", C.c_int64), ("timeout_ns", C.c_int64), ("time_limit_ns", C.c_int64)]
+
+
 class NemesisConfig(C.Structure):   # ms_nemesis_config
     _fields_ = [("group", C.c_uint32), ("targets", C.c_uint32), ("interval_ns", C.c_int64), ("start_ns", C.c_int64),
                 ("time_limit_ns", C.c_int64)]
@@ -63,6 +68,10 @@ class NemesisConfig(C.Structure):   # ms_nemesis_config
 HIST_DTYPE = np.dtype([("time_ns", "<i8"), ("order", "<u8"), ("client", "<u4"), ("op", "<u4"), ("type", "u1"),
                        ("f", "u1"), ("error", "<u2"), ("value", "<u4")])
 assert HIST_DTYPE.itemsize == 32
+KAFKA_HIST_DTYPE = np.dtype([("time_ns", "<i8"), ("order", "<u8"), ("client", "<u4"), ("op", "<u4"), ("type", "u1"),
+                             ("f", "u1"), ("error", "<u2"), ("key", "<u4", (2,)), ("a", "<u4", (2,)), ("b", "<u4", (2,)),
+                             ("pad", "<u4", (3,))])
+assert KAFKA_HIST_DTYPE.itemsize == 64
 
 
 class JBatch(C.Structure):      # ms_jbatch
@@ -95,6 +104,10 @@ SYMBOLS = {
     "ms_add_gen_clients": (C.c_int, [_P, _P, C.c_uint32]),
     "ms_add_kv_clients": (C.c_int, [_P, _P, C.c_uint32]),
     "ms_history_drain": (C.c_int, [_P, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "ms_add_kafka_clients": (C.c_int, [_P, _P, C.c_uint32]),
+    "ms_kafka_history_drain": (C.c_int, [_P, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "ms_kafka_log": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "ms_kafka_committed": (C.c_int64, [_P, C.c_uint32, C.c_uint32]),
     "ms_schedule_ops": (C.c_int, [_P, _P, C.c_size_t]),
     "ms_step": (C.c_int, [_P, C.c_uint64]),
     "ms_run": (C.c_int, [_P, C.c_int64]),

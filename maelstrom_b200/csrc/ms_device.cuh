@@ -22,7 +22,7 @@ enum : uint32_t {
   E_NONE = 0, E_RING_OVERFLOW = 1, E_WINDOW_OVERFLOW = 2, E_JOURNAL_OVERFLOW = 3,
   E_INVALID_DEST = 4, E_HISTORY = 5, E_VALUE_RANGE = 6, E_MAIL_OVERFLOW = 7,
   E_CALENDAR_OVERFLOW = 8, E_ID_RANGE = 9, E_BARRIER = 10, E_SNAPSHOT = 11,
-  E_RAFT_CAPACITY = 12, E_HISTORY_RING = 13
+  E_RAFT_CAPACITY = 12, E_HISTORY_RING = 13, E_KAFKA_CAPACITY = 14
 };
 
 // Mutable per-simulation scalars, resident in HBM, committed by the last CTA of
@@ -81,6 +81,9 @@ struct DevState {
   // partition nemesis (ms_set_nemesis): the earliest instant at which some cluster acts (nem_pending); k_nemesis
   // returns at once before it.  Appended
   int64_t  nem_next;
+  // kafka clients (ms_add_kafka_clients): their own ring of 64-B history records, as gc_hist_n / _drained.  Appended
+  uint64_t kf_hist_n;
+  uint64_t kf_hist_drained;
 };
 
 // One row per round, kept in a ring of `hist` rounds: what is needed to turn an
@@ -256,6 +259,15 @@ struct Params {
   int64_t   nem_interval_ns, nem_limit_ns;
   // MS_W_KV_PROXY (kp_handle in csrc/ms_raft.cuh): the backing service, MS_SVC_*.  Appended
   uint32_t  kp_service, kp_pad;
+  // MS_W_KAFKA (kf_handle in csrc/ms_raft.cuh): per node and key the log, its length and the committed offset
+  // (kKafkaAbsent = none); the kafka clients' state beside their GenDev and their history ring.  Appended
+  uint32_t* kf_log;          // [n_servers][kf_keys][kf_cap] messages
+  uint32_t* kf_len;          // [n_servers][kf_keys]
+  uint32_t* kf_committed;    // [n_servers][kf_keys]
+  uint32_t  kf_keys, kf_cap;
+  struct KfGenDev* kf_gc;    // [max_endpoints], valid where gc is a kafka client's
+  uint4*    kf_hist;         // ring of 64-B ms_kafka_hist records
+  uint32_t  kf_hist_mask, kf_assign_permille, kf_crash_permille, kf_pad;
 };
 
 constexpr uint32_t kRaftCallbacks = 4096;       // default pending-RPC table slots per node (ms_config.reserved[5]; oracle: same)
@@ -308,6 +320,19 @@ struct GenDev {
   uint32_t reader;                     // lin-kv client: 1 = only reads (gen/reserve)
 };
 enum : uint32_t { GEN_MIX = 0, GEN_QUIET = 1, GEN_FINAL = 2, GEN_DONE = 3 };
+
+// kafka client (ms_add_kafka_clients): what the Client record of workload/kafka.clj:191-241 keeps beyond GenDev (whose
+// bcasts counts its sends).  key / off: the assignment and the local offsets (:197 `offsets`); the op in flight has
+// its history slots in hkey / ha / hb and waits for the reply of request `sub`
+constexpr uint32_t kKafkaNoKey = 0xFFFFu;
+constexpr uint32_t kKafkaAbsent = 0xFFFFFFFFu;
+enum : uint32_t { KF_IDLE = 0, KF_LIST = 1, KF_SEND = 2, KF_POLL = 3, KF_COMMIT = 4 };
+struct KfGenDev {
+  uint32_t key[2], off[2];
+  uint32_t sub;
+  uint32_t hkey[2], ha[2], hb[2];
+  uint32_t pad;
+};
 
 constexpr uint32_t kSeqBuffer = 32;             // (sequential 32 ...), service.clj:206-208
 constexpr uint32_t kSeqHist = kSeqBuffer + 1;   // versions per key that can matter to a resident state

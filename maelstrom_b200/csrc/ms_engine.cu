@@ -94,6 +94,7 @@ static const char* dev_error_text(uint32_t code) {
     case E_ID_RANGE: return "per-ticket count exceeds the table entry range at ticket";
     case E_BARRIER: return "cross-shard barrier timed out waiting for shard";
     case E_RAFT_CAPACITY: return "Raft node out of log / staging / payload-heap capacity (raise ms_config.reserved[3]) at node";
+    case E_KAFKA_CAPACITY: return "kafka node's log of a key is full (raise ms_config.reserved[3]) at node";
     case E_HISTORY_RING: return "history ring of the closed-loop clients is full (call ms_history_drain more often) at client";
     case E_SNAPSHOT: return "replicate_full names a set snapshot that is not resident (in flight longer than calendar_slots, or forged): sender";
   }
@@ -599,7 +600,7 @@ static int build_sim(ms_sim* s, const ms_config* in) {
   ms_config& c = s->cfg;
   c = *in;
   if (c.n_nodes == 0) { set_err("n_nodes must be positive (--node-count)"); return MS_ERR_ARG; }
-  if (c.workload > MS_W_KV_PROXY || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
+  if (c.workload > MS_W_KAFKA || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
     set_err("bad workload/topology/latency_dist");
     return MS_ERR_ARG;
   }
@@ -796,6 +797,23 @@ static int build_sim(ms_sim* s, const ms_config* in) {
     P.kp_service = c.reserved[3];
     P.rf_n_keys = c.reserved[2] ? c.reserved[2] : 4096u;           // the service's keys bound the clients' key ranges
     P.rf_group = (c.reserved[4] && c.reserved[4] < c.n_nodes) ? c.reserved[4] : 0u;
+  }
+  if (c.workload == MS_W_KAFKA) {
+    // single-node kafka logs (kf_handle, csrc/ms_raft.cuh): per node and key the log, its length and the committed
+    // offset; the staging rows of the sequential step (one reply per message received), no closures
+    if (c.n_shards > 1) { set_err("MS_W_KAFKA runs on one GPU"); return MS_ERR_ARG; }
+    P.kf_keys = c.reserved[2] ? c.reserved[2] : 16u;
+    P.kf_cap = c.reserved[3] ? c.reserved[3] : 4096u;
+    if (P.kf_keys > 65535u) { set_err("MS_W_KAFKA: ms_config.reserved[2] (keys per node) must be <= 65535"); return MS_ERR_ARG; }
+    const size_t N = c.n_nodes;
+    P.rf_stage_cap = c.server_max_window + 16u;
+    P.rf_cb_mask = 0;
+    if ((rc = s->dalloc(&P.rf_node, N)) || (rc = s->dalloc(&P.rf_cb, N * 2)) || (rc = s->dalloc(&P.rf_stage, N * P.rf_stage_cap * 3)) ||
+        (rc = s->dalloc(&P.kf_log, N * P.kf_keys * P.kf_cap)) || (rc = s->dalloc(&P.kf_len, N * P.kf_keys)) ||
+        (rc = s->dalloc(&P.kf_committed, N * P.kf_keys)))
+      return rc;
+    CK(cudaMemsetAsync(P.kf_committed, 0xFF, N * P.kf_keys * 4, s->stream));   // kKafkaAbsent: nothing committed
+    CK(cudaStreamSynchronize(s->stream));
   }
   if (c.workload == MS_W_TXN || c.workload == MS_W_TXN_TREE || c.workload == MS_W_KV_PROXY) {
     // txn-list-append nodes and lin-kv proxies: message ids, the table of pending RPC closures and the staging rows
@@ -1199,6 +1217,123 @@ int ms_add_kv_clients(ms_sim* s, const ms_kv_gen_config* kc, uint32_t first_name
   CK(cudaMemcpy(P.kind + first, s->kinds.data() + first, kc->n_clients, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(P.gc + first, init.data(), init.size() * sizeof(GenDev), cudaMemcpyHostToDevice));
   return (int)first;
+}
+
+// Closed-loop kafka clients of the single-node logs: n endpoints "c<first_name>..", client k on server k mod n, driven
+// by kf_gen_step inside the sequential family's round kernel (csrc/ms_kernels.cu).
+int ms_add_kafka_clients(ms_sim* s, const ms_kafka_gen_config* kc, uint32_t first_name) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  if (!kc || kc->n_clients == 0 || kc->interval_ns <= 0 || kc->timeout_ns < 0 ||
+      (uint64_t)kc->assign_permille + kc->crash_permille > 1000) {
+    set_err("ms_add_kafka_clients: bad configuration");
+    return MS_ERR_ARG;
+  }
+  if (s->cfg.workload != MS_W_KAFKA) { set_err("ms_add_kafka_clients: the kafka clients drive the kafka nodes (MS_W_KAFKA)"); return MS_ERR_ARG; }
+  if (s->P.gc) { set_err("ms_add_kafka_clients: the generator's clients exist already"); return MS_ERR_ARG; }
+  if (kc->n_clients % s->cfg.n_nodes) {
+    set_err("ms_add_kafka_clients: n_clients must be a multiple of n_nodes (" + std::to_string(s->cfg.n_nodes) + ")");
+    return MS_ERR_ARG;
+  }
+  Params& P = s->P;
+  if ((uint64_t)P.n_ep + kc->n_clients > s->cfg.max_endpoints) { set_err("max_endpoints exhausted"); return MS_ERR_CAPACITY; }
+  for (uint32_t k = 0; k < kc->n_clients; k++)
+    if (s->by_name.count("c" + std::to_string(first_name + k))) { set_err("endpoint already exists: c" + std::to_string(first_name + k)); return MS_ERR_ARG; }
+  int rc;
+  // an op writes at most two records per round (a crash; or a completion and the next invocation)
+  const uint32_t hist_cap = pow2_at_least(std::max<uint32_t>(1u << 16, 64u * kc->n_clients));
+  if ((rc = s->dalloc(&P.gc, s->cfg.max_endpoints)) || (rc = s->dalloc(&P.kf_gc, s->cfg.max_endpoints)) ||
+      (rc = s->dalloc(&P.kf_hist, (size_t)hist_cap * 4)))
+    return rc;
+  P.kf_hist_mask = hist_cap - 1u;
+  P.gc_n = kc->n_clients;
+  P.gc_interval_ns = kc->interval_ns;
+  P.gc_timeout_ns = kc->timeout_ns > 0 ? kc->timeout_ns : 5000ll * kTickNs;      // client.clj:18-20
+  P.gc_limit_ns = kc->time_limit_ns;
+  P.kf_assign_permille = kc->assign_permille;
+  P.kf_crash_permille = kc->crash_permille;
+  const uint32_t first = P.n_ep;
+  std::vector<GenDev> init(kc->n_clients);
+  std::vector<KfGenDev> kinit(kc->n_clients);
+  memset(init.data(), 0, init.size() * sizeof(GenDev));
+  memset(kinit.data(), 0, kinit.size() * sizeof(KfGenDev));
+  for (uint32_t k = 0; k < kc->n_clients; k++) {
+    const std::string id = "c" + std::to_string(first_name + k);
+    const uint32_t idx = first + k;
+    s->kinds[idx] = MS_KIND_GEN_CLIENT;
+    s->names.push_back(id);
+    s->mailbox.emplace_back();
+    s->by_name[id] = idx;
+    init[k].node = k % s->cfg.n_nodes;
+    init[k].ordinal = k;
+    kinit[k].key[0] = kinit[k].key[1] = kKafkaNoKey;
+  }
+  P.n_ep = first + kc->n_clients;
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(P.kind + first, s->kinds.data() + first, kc->n_clients, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(P.gc + first, init.data(), init.size() * sizeof(GenDev), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(P.kf_gc + first, kinit.data(), kinit.size() * sizeof(KfGenDev), cudaMemcpyHostToDevice));
+  return (int)first;
+}
+
+int ms_kafka_history_drain(ms_sim* s, ms_kafka_hist* out, size_t cap, size_t* n_out) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  if (n_out) *n_out = 0;
+  if (!s->P.kf_hist) return MS_OK;
+  const uint64_t avail = s->hs.kf_hist_n - s->hs.kf_hist_drained;
+  const size_t n = (size_t)std::min<uint64_t>(avail, cap);
+  if (!n || !out) return MS_OK;
+  static_assert(sizeof(ms_kafka_hist) == 64, "ms_kafka_hist is the device record");
+  for (size_t k = 0; k < n;) {      // the ring may wrap
+    const uint64_t pos = (s->hs.kf_hist_drained + k) & s->P.kf_hist_mask;
+    const size_t piece = (size_t)std::min<uint64_t>(n - k, (uint64_t)s->P.kf_hist_mask + 1 - pos);
+    CK(cudaMemcpy(out + k, s->P.kf_hist + pos * 4, piece * 64, cudaMemcpyDeviceToHost));
+    k += piece;
+  }
+  // as ms_history_drain: (time, round, client) is the order; one client's records of a round keep theirs
+  std::stable_sort(out, out + n, [](const ms_kafka_hist& a, const ms_kafka_hist& b) {
+    return a.time_ns != b.time_ns ? a.time_ns < b.time_ns : a.order < b.order;
+  });
+  s->hs.kf_hist_drained += n;
+  CK(cudaMemcpy(&s->P.st->kf_hist_drained, &s->hs.kf_hist_drained, 8, cudaMemcpyHostToDevice));
+  if (n_out) *n_out = n;
+  return MS_OK;
+}
+
+static int kafka_slot(ms_sim* s, uint32_t node, uint32_t key, const char* what) {
+  if (s->cfg.workload != MS_W_KAFKA || node >= s->cfg.n_nodes || key >= s->P.kf_keys) {
+    set_err(std::string(what) + ": not a kafka node or key (MS_W_KAFKA, node < n_nodes, key < ms_config.reserved[2])");
+    return MS_ERR_ARG;
+  }
+  return MS_OK;
+}
+
+int ms_kafka_log(ms_sim* s, uint32_t node, uint32_t key, uint32_t* msgs, size_t cap, size_t* len) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  if (len) *len = 0;
+  int rc;
+  if ((rc = kafka_slot(s, node, key, "ms_kafka_log"))) return rc;
+  const size_t row = (size_t)node * s->P.kf_keys + key;
+  uint32_t n = 0;
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(&n, s->P.kf_len + row, 4, cudaMemcpyDeviceToHost));
+  const size_t m = std::min<size_t>(n, msgs ? cap : 0);
+  if (m) CK(cudaMemcpy(msgs, s->P.kf_log + row * s->P.kf_cap, m * 4, cudaMemcpyDeviceToHost));
+  if (len) *len = n;
+  return MS_OK;
+}
+
+int64_t ms_kafka_committed(ms_sim* s, uint32_t node, uint32_t key) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  int rc;
+  if ((rc = kafka_slot(s, node, key, "ms_kafka_committed"))) return rc;
+  uint32_t c = 0;
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(&c, s->P.kf_committed + (size_t)node * s->P.kf_keys + key, 4, cudaMemcpyDeviceToHost));
+  return c == kKafkaAbsent ? -1 : (int64_t)c;
 }
 
 int ms_history_drain(ms_sim* s, ms_hist* out, size_t cap, size_t* n_out) {
@@ -2080,7 +2215,7 @@ uint64_t ms_undeliverable(ms_sim* s) { std::lock_guard<std::mutex> g(s->mu); ret
 int ms_raft_state(ms_sim* s, uint32_t node, uint64_t out[8]) {
   std::lock_guard<std::mutex> g(s->mu);
   cudaSetDevice(s->device);
-  if (!s->P.rf_node || node >= s->cfg.n_nodes) { set_err("ms_raft_state: not a Raft node"); return MS_ERR_ARG; }
+  if (!s->P.rf_node || node >= s->cfg.n_nodes || s->cfg.workload == MS_W_KAFKA) { set_err("ms_raft_state: not a Raft node"); return MS_ERR_ARG; }
   RaftDev r;
   CK(cudaStreamSynchronize(s->stream));
   CK(cudaMemcpy(&r, s->P.rf_node + node, sizeof r, cudaMemcpyDeviceToHost));

@@ -102,6 +102,18 @@ jlong FN(historyDrain)(JNIEnv* env, jclass c, jlong h, jobject out, jlong cap) {
   const int rc = ms_history_drain(H(h), (ms_hist*)BUF(out), (size_t)cap, &n);
   return rc < 0 ? (jlong)rc : (jlong)n;
 }
+/* the kafka clients of the single-node logs: cfg = direct buffer holding an ms_kafka_gen_config; records are
+ * ms_kafka_hist (64 B) */
+jint FN(addKafkaClients)(JNIEnv* env, jclass c, jlong h, jobject cfg, jint firstName) {
+  (void)c;
+  return ms_add_kafka_clients(H(h), (const ms_kafka_gen_config*)BUF(cfg), (uint32_t)firstName);
+}
+jlong FN(kafkaHistoryDrain)(JNIEnv* env, jclass c, jlong h, jobject out, jlong cap) {
+  (void)c;
+  size_t n = 0;
+  const int rc = ms_kafka_history_drain(H(h), (ms_kafka_hist*)BUF(out), (size_t)cap, &n);
+  return rc < 0 ? (jlong)rc : (jlong)n;
+}
 jint FN(scheduleOps)(JNIEnv* env, jclass c, jlong h, jobject ops, jlong n) {
   (void)c;
   return ms_schedule_ops(H(h), (const ms_op*)BUF(ops), (size_t)n);
@@ -203,6 +215,14 @@ jlong FN(nodeSet)(JNIEnv* env, jclass c, jlong h, jint node, jobject values, jlo
 jlong FN(clientReplies)(JNIEnv* env, jclass c, jlong h) { (void)env; (void)c; return (jlong)ms_client_replies(H(h)); }
 jlong FN(undeliverable)(JNIEnv* env, jclass c, jlong h) { (void)env; (void)c; return (jlong)ms_undeliverable(H(h)); }
 jint FN(raftState)(JNIEnv* env, jclass c, jlong h, jint node, jobject out8) { (void)c; return ms_raft_state(H(h), (uint32_t)node, (uint64_t*)BUF(out8)); }
+/* kafka read-backs: msgs = direct buffer of cap u32; returns the log's length or a negative error */
+jlong FN(kafkaLog)(JNIEnv* env, jclass c, jlong h, jint node, jint key, jobject msgs, jlong cap) {
+  (void)c;
+  size_t n = 0;
+  const int rc = ms_kafka_log(H(h), (uint32_t)node, (uint32_t)key, msgs ? (uint32_t*)BUF(msgs) : NULL, (size_t)cap, &n);
+  return rc < 0 ? (jlong)rc : (jlong)n;
+}
+jlong FN(kafkaCommitted)(JNIEnv* env, jclass c, jlong h, jint node, jint key) { (void)env; (void)c; return ms_kafka_committed(H(h), (uint32_t)node, (uint32_t)key); }
 jint FN(counters)(JNIEnv* env, jclass c, jlong h, jobject out8) { (void)c; return ms_counters(H(h), (uint64_t*)BUF(out8)); }
 /* out = direct buffer of n u64 (>= 6 x n_nodes): tail / limit / head of the 48-B rings, then of the compact rings */
 jint FN(ringCounters)(JNIEnv* env, jclass c, jlong h, jobject out, jint n) { (void)c; return ms_ring_counters(H(h), (uint64_t*)BUF(out), (uint32_t)n); }

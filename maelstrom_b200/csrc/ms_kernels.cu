@@ -601,6 +601,163 @@ __device__ bool kv_gen_step(const Params& p, DevState* st, uint32_t e, int64_t n
   return send;
 }
 
+// The kafka client (ms_add_kafka_clients, DESIGN.md 2.15): the client side of kv_gen_step with the Client of
+// workload/kafka.clj:191-241 and the generator of the header; the oracle's twin is tests/native/kafka_oracle.cpp.
+// The extra state is p.kf_gc[e]; the GenDev fields keep their meaning (bcasts counts the sends), so gen_timer_due
+// and gen_wake_ns hold for it as they are: a commit goes out on the poll_ok, a crash completes at once.
+__device__ void kf_hist(const Params& p, DevState* st, int64_t now, uint64_t round, uint32_t e, const GenDev& g,
+                        const KfGenDev& k, uint32_t type, uint32_t f, uint32_t error) {
+  const unsigned long long pos = atomicAdd((unsigned long long*)&st->kf_hist_n, 1ull);
+  if (pos - st->kf_hist_drained > p.kf_hist_mask) { latch_error(st, E_HISTORY_RING, e); return; }
+  uint4* at = p.kf_hist + (pos & p.kf_hist_mask) * 4;
+  const uint64_t order = (round << 24) | g.ordinal;
+  at[0] = make_uint4((uint32_t)now, (uint32_t)((uint64_t)now >> 32), (uint32_t)order, (uint32_t)(order >> 32));
+  at[1] = make_uint4(e, g.ops, type | (f << 8) | (error << 16), k.hkey[0]);
+  at[2] = make_uint4(k.hkey[1], k.ha[0], k.ha[1], k.hb[0]);
+  at[3] = make_uint4(k.hb[1], 0u, 0u, 0u);
+}
+
+__device__ __forceinline__ void kf_reopen(KfGenDev& k) {      // a fresh Client: (atom {}) of open! (:193-198)
+  k.key[0] = k.key[1] = kKafkaNoKey;
+  k.off[0] = k.off[1] = 0;
+}
+
+__device__ bool kf_gen_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const uint4* myring,
+                            uint32_t head, uint32_t my_mask, uint32_t n, const uint16_t* ord, const uint32_t* vals, Rec& out) {
+  GenDev g = p.gc[e];
+  KfGenDev k = p.kf_gc[e];
+  bool send = false;
+  for (uint32_t pos = 0; pos < n; pos++) {
+    const uint32_t i = ord[pos];
+    if (!(vals[i] & (1u << 30))) continue;                                 // V_RECV: cut by a partition
+    const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
+    const uint4 vb = rp[1], vc = rp[2];
+    const uint32_t type = vc.x & 0xFFFFu, flags = vc.x >> 16;
+    if (!g.waiting_for || !(flags & MS_F_REPLY) || vb.w != g.waiting_for) continue;   // client.clj:106-107
+    g.waiting_for = 0;
+    if (type == MS_T_ERROR) {                                              // with-errors #{:assign} (:202)
+      const uint32_t err = vc.y;
+      const bool info = k.sub != KF_LIST && (err == 0 || err == 13);
+      kf_hist(p, st, now, round, e, g, k, info ? MS_H_INFO : MS_H_FAIL, g.cur_f, err);
+      if (info) kf_reopen(k);
+      k.sub = KF_IDLE;
+      continue;
+    }
+    const uint32_t rkeys = vc.y;
+    const uint64_t rp1 = (uint64_t)vc.z | ((uint64_t)vc.w << 32);
+    if (k.sub == KF_LIST) {                                                // assign: local, else committed, else 0
+      for (int s = 0; s < 2; s++) {
+        const uint32_t key = k.hkey[s];
+        if (key == kKafkaNoKey) continue;
+        uint32_t start = 0, comm = kKafkaAbsent;
+        for (int r = 0; r < 2; r++)
+          if (((rkeys >> (16 * r)) & 0xFFFFu) == key) comm = (uint32_t)(rp1 >> (32 * r));
+        if (comm != kKafkaAbsent) start = comm;
+        for (int l = 0; l < 2; l++)
+          if (k.key[l] == key) start = k.off[l];
+        k.ha[s] = start; k.hb[s] = comm;
+      }
+      for (int s = 0; s < 2; s++) { k.key[s] = k.hkey[s]; k.off[s] = k.ha[s]; }
+      kf_hist(p, st, now, round, e, g, k, MS_H_OK, g.cur_f, 0);
+      k.sub = KF_IDLE;
+    } else if (k.sub == KF_SEND) {
+      k.hb[0] = (uint32_t)rp1;                                             // send_ok's offset
+      kf_hist(p, st, now, round, e, g, k, MS_H_OK, g.cur_f, 0);
+      k.sub = KF_IDLE;
+    } else if (k.sub == KF_POLL) {                                         // apply-mop! :poll (:166-182)
+      uint32_t commit_keys = 0xFFFFFFFFu;
+      uint64_t commit_offs = 0;
+      for (int s = 0; s < 2; s++) {
+        const uint32_t key = (rkeys >> (16 * s)) & 0xFFFFu, len = (uint32_t)(rp1 >> (32 * s));
+        k.hkey[s] = key;
+        if (key == kKafkaNoKey) { k.ha[s] = 0; k.hb[s] = 0; continue; }
+        k.hb[s] = len;                                                     // ha keeps the offset asked for: the first
+        if (k.key[s] == key && len > k.off[s]) k.off[s] = len;             // merge-with max of (inc highest offset)
+        commit_keys = (commit_keys & ~(0xFFFFu << (16 * s))) | (key << (16 * s));
+        commit_offs |= (uint64_t)(len - 1u) << (32 * s);                  // txn-offsets: the highest offset polled
+      }
+      if (commit_keys == 0xFFFFFFFFu) {                                    // nothing polled: nothing to commit
+        kf_hist(p, st, now, round, e, g, k, MS_H_OK, g.cur_f, 0);
+        k.sub = KF_IDLE;
+      } else {                                                             // commit_offsets! (:228-231)
+        k.sub = KF_COMMIT;
+        g.waiting_for = ++g.next_msg_id;
+        g.deadline_ns = now + p.gc_timeout_ns;
+        out.round = 0; out.ticket = 0; out.idx = 0;
+        out.src = e; out.dest = g.node; out.msg_id = g.waiting_for; out.in_reply_to = 0;
+        out.tf = MS_T_COMMIT_OFFSETS | ((uint32_t)MS_F_MSG_ID << 16);
+        out.p0 = commit_keys; out.p1 = commit_offs;
+        send = true;
+      }
+    } else {                                                               // KF_COMMIT: the poll completes
+      kf_hist(p, st, now, round, e, g, k, MS_H_OK, g.cur_f, 0);
+      k.sub = KF_IDLE;
+    }
+  }
+  if (g.waiting_for && now >= g.deadline_ns) {                             // :net-timeout
+    const bool info = k.sub != KF_LIST;
+    kf_hist(p, st, now, round, e, g, k, info ? MS_H_INFO : MS_H_FAIL, g.cur_f, MS_H_TIMEOUT);
+    if (info) kf_reopen(k);
+    k.sub = KF_IDLE;
+    g.waiting_for = 0;
+  }
+  if (!g.waiting_for && g.phase == GEN_MIX) {
+    if (now >= p.gc_limit_ns) {
+      g.phase = GEN_DONE;
+    } else if (now >= g.next_op_ns) {
+      uint32_t x[4];
+      philox4x32_10(g.ops, e, 0xC11E47u, 0u, p.seed_lo, p.seed_hi, x);     // the client's own stream: op k
+      const uint32_t K = p.kf_keys;
+      const uint32_t r = (uint32_t)(((uint64_t)x[0] * 1000u) >> 32);
+      g.next_op_ns = now + (int64_t)(((unsigned __int128)x[1] * (unsigned __int128)(2 * (uint64_t)p.gc_interval_ns)) >> 32);
+      g.ops++;
+      const uint32_t k0 = (uint32_t)(((uint64_t)x[2] * K) >> 32);
+      k.hkey[0] = k.hkey[1] = kKafkaNoKey;
+      k.ha[0] = k.ha[1] = k.hb[0] = k.hb[1] = 0;
+      out.round = 0; out.ticket = 0; out.idx = 0;
+      out.src = e; out.dest = g.node; out.in_reply_to = 0;
+      if (r < p.kf_assign_permille) {                                      // :assign, then list_committed_offsets
+        g.cur_f = MS_HF_KAFKA_ASSIGN;
+        k.hkey[0] = k0;
+        if (K >= 2 && (x[3] & 1u)) k.hkey[1] = (k0 + 1u + (uint32_t)(((uint64_t)x[3] * (K - 1u)) >> 32)) % K;
+        k.sub = KF_LIST;
+        out.tf = MS_T_LIST_COMMITTED_OFFSETS;
+        out.p0 = k.hkey[0] | (k.hkey[1] << 16); out.p1 = 0;
+        send = true;
+      } else if (r < p.kf_assign_permille + p.kf_crash_permille) {         // :crash, :info at once; the client reopens
+        g.cur_f = MS_HF_KAFKA_CRASH;
+        kf_hist(p, st, now, round, e, g, k, MS_H_INVOKE, g.cur_f, 0);
+        kf_hist(p, st, now, round, e, g, k, MS_H_INFO, g.cur_f, 0);
+        kf_reopen(k);
+      } else if (!(x[3] & 1u)) {                                           // send! (:184-186)
+        g.cur_f = MS_HF_KAFKA_SEND;
+        k.hkey[0] = k0; k.ha[0] = g.ordinal + p.gc_n * g.bcasts++; k.hb[0] = kKafkaAbsent;
+        k.sub = KF_SEND;
+        out.tf = MS_T_SEND;
+        out.p0 = k0; out.p1 = k.ha[0];
+        send = true;
+      } else {                                                             // poll at the local offsets
+        g.cur_f = MS_HF_KAFKA_POLL;
+        for (int s = 0; s < 2; s++) { k.hkey[s] = k.key[s]; k.ha[s] = k.key[s] == kKafkaNoKey ? 0u : k.off[s]; }
+        k.sub = KF_POLL;
+        out.tf = MS_T_POLL;
+        out.p0 = k.hkey[0] | (k.hkey[1] << 16); out.p1 = (uint64_t)k.ha[0] | ((uint64_t)k.ha[1] << 32);
+        send = true;
+      }
+      if (send) {
+        kf_hist(p, st, now, round, e, g, k, MS_H_INVOKE, g.cur_f, 0);
+        g.waiting_for = ++g.next_msg_id;                                   // client.clj:61-64
+        g.deadline_ns = now + p.gc_timeout_ns;
+        out.msg_id = g.waiting_for;
+        out.tf |= (uint32_t)MS_F_MSG_ID << 16;
+      }
+    }
+  }
+  p.gc[e] = g;
+  p.kf_gc[e] = k;
+  return send;
+}
+
 #include "ms_tree.h"
 #include "ms_raft.cuh"
 
@@ -1631,7 +1788,7 @@ __device__ void service_handle(const Params& p, uint32_t svc, const SvReq& q, ui
 }
 
 // ------------------------------------------------------------------ node programs run by k_round
-// Raft / txn-list-append server e (ms_raft.cuh), one thread: the window in id order, then the node's timers.
+// Raft / txn-list-append / proxy / kafka server e (ms_raft.cuh), one thread: the window in id order, then the node's timers.
 // Returns the number of sends it staged in rf_stage; k_round emits them.
 __device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const Win& w,
                               uint32_t n, const RoundSmem& sm) {
@@ -1645,6 +1802,7 @@ __device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t
     if (p.workload == MS_W_RAFT) rf_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else if (p.workload == MS_W_TXN_TREE) tt_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else if (p.workload == MS_W_KV_PROXY) kp_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+    else if (p.workload == MS_W_KAFKA) kf_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else txn_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
   }
   if (p.workload == MS_W_RAFT) { rf_actions(c); rf_note_busy(c); }
@@ -2228,8 +2386,10 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       if (tid == 0) {
         Rec q;
         bool send;
-        // the Raft family's clients are the lin-kv ones (ms_add_kv_clients); their requests carry a p1
-        if constexpr (RF) send = kv_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
+        // the Raft family's clients are the lin-kv ones (ms_add_kv_clients) or the kafka ones (ms_add_kafka_clients);
+        // their requests carry a p1
+        if constexpr (RF) send = p.workload == MS_W_KAFKA ? kf_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q)
+                                                          : kv_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
         else send = gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
         if (send) {
           s_gen[0] = make_uint4(q.src, q.dest, q.msg_id, q.in_reply_to);

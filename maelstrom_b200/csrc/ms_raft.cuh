@@ -528,6 +528,82 @@ __device__ void kp_handle(RaftCtx& c, const Rec& m) {
   r->state = 1;                                                                   // "No handler": main! raises, node.rb:167
 }
 
+// ------------------------------------------------------------------ kafka, single node
+// demo/clojure/kafka_single_node.clj (DESIGN.md 2.15): every node keeps its own append-only log per key
+// (Params.kf_log / kf_len) and committed offsets (kf_committed, kKafkaAbsent = none).  Handlers run in dequeue
+// order, a legal schedule of the demo's future per message.  A poll_ok carries the log lengths, not the messages:
+// the log never changes below its length, so ms_kafka_log gives them afterwards.  Keys of a request are checked
+// before any effect; slot 0 is applied before slot 1.
+__device__ __forceinline__ bool kf_keys_ok(RaftCtx& c, uint32_t keys) {
+  for (int i = 0; i < 2; i++) {
+    const uint32_t k = (keys >> (16 * i)) & 0xFFFFu;
+    if (k != kKafkaNoKey && k >= c.p.kf_keys) { latch_error(c.st, E_VALUE_RANGE, k); return false; }
+  }
+  return true;
+}
+
+__device__ void kf_handle(RaftCtx& c, const Rec& m) {
+  const uint32_t type = m.tf & 0xFFFFu, flags = m.tf >> 16;
+  if (flags & MS_F_REPLY) return;                                                 // handle-reply!: no rpcs of its own (:80-88)
+  const bool has_id = (flags & MS_F_MSG_ID) != 0;
+  Rec a;                                                                          // reply! (:65-68)
+  a.round = 0; a.ticket = 0; a.idx = 0;
+  a.src = c.e; a.dest = m.src; a.msg_id = 0;
+  a.in_reply_to = has_id ? m.msg_id : 0u;                                         // in_reply_to: nil without a msg_id
+  a.p0 = 0; a.p1 = 0;
+  const size_t row = (size_t)c.e * c.p.kf_keys;
+  uint32_t* len = c.p.kf_len + row;
+  uint32_t* committed = c.p.kf_committed + row;
+  uint32_t out_type = MS_T_ERROR;
+  if (type == MS_T_INIT) {                                                        // handle-init! (:90-97)
+    out_type = MS_T_INIT_OK;
+  } else if (type == MS_T_SEND) {                                                 // handle-send! (:197-207)
+    const uint32_t k = m.p0;
+    if (k >= c.p.kf_keys) { latch_error(c.st, E_VALUE_RANGE, k); return; }
+    const uint32_t n = len[k];
+    if (n >= c.p.kf_cap) { latch_error(c.st, E_KAFKA_CAPACITY, c.e); return; }
+    c.p.kf_log[(row + k) * c.p.kf_cap + n] = (uint32_t)m.p1;
+    len[k] = n + 1u;
+    out_type = MS_T_SEND_OK;
+    a.p1 = n;                                                                     // (dec (count queue'))
+  } else if (type == MS_T_POLL) {                                                 // handle-poll! (:174-195)
+    if (!kf_keys_ok(c, m.p0)) return;
+    uint32_t keys = 0xFFFFFFFFu;
+    for (int i = 0; i < 2; i++) {
+      const uint32_t k = (m.p0 >> (16 * i)) & 0xFFFFu, o = (uint32_t)(m.p1 >> (32 * i));
+      if (k == kKafkaNoKey || o >= len[k]) continue;                              // (min offset (count queue)): no msgs, omitted
+      keys = (keys & ~(0xFFFFu << (16 * i))) | (k << (16 * i));
+      a.p1 |= (uint64_t)len[k] << (32 * i);
+    }
+    out_type = MS_T_POLL_OK;
+    a.p0 = keys;
+  } else if (type == MS_T_COMMIT_OFFSETS) {                                       // merge-with max (:159-165)
+    if (!kf_keys_ok(c, m.p0)) return;
+    for (int i = 0; i < 2; i++) {
+      const uint32_t k = (m.p0 >> (16 * i)) & 0xFFFFu, o = (uint32_t)(m.p1 >> (32 * i));
+      if (k == kKafkaNoKey) continue;
+      if (o == kKafkaAbsent) { latch_error(c.st, E_VALUE_RANGE, o); return; }
+      if (committed[k] == kKafkaAbsent || o > committed[k]) committed[k] = o;
+    }
+    out_type = MS_T_COMMIT_OFFSETS_OK;
+  } else if (type == MS_T_LIST_COMMITTED_OFFSETS) {                               // select-keys (:167-172)
+    if (!kf_keys_ok(c, m.p0)) return;
+    uint32_t keys = 0xFFFFFFFFu;
+    for (int i = 0; i < 2; i++) {
+      const uint32_t k = (m.p0 >> (16 * i)) & 0xFFFFu;
+      if (k == kKafkaNoKey || committed[k] == kKafkaAbsent) continue;
+      keys = (keys & ~(0xFFFFu << (16 * i))) | (k << (16 * i));
+      a.p1 |= (uint64_t)committed[k] << (32 * i);
+    }
+    out_type = MS_T_LIST_COMMITTED_OFFSETS_OK;
+    a.p0 = keys;
+  } else {
+    a.p0 = 10;                                                                    // "Unknown request type", {:code 10}
+  }
+  a.tf = out_type | ((has_id ? (uint32_t)MS_F_REPLY : 0u) << 16);
+  rf_emit(c, a);
+}
+
 // ------------------------------------------------------------------ txn-list-append on a persistent hash tree
 // demo/ruby/datomic_list_append.rb.  The database is a tree of immutable nodes stored in lww-kv under
 // unique pointers; lin-kv holds the pointer to the root (key "root" = key 0 here).  A txn (:340-353, under

@@ -9,7 +9,7 @@ from . import _lib
 from ._lib import Body, Config, EVENT_DTYPE, JBODY_DTYPE, MSG_DTYPE, OP_DTYPE  # noqa: F401
 
 WORKLOADS = {"echo": 0, "broadcast": 1, "g-set": 2, "lin-kv": 3, "txn-list-append": 4, "txn-list-append-tree": 5,
-             "lin-kv-proxy": 6}
+             "lin-kv-proxy": 6, "kafka": 7}
 TOPOLOGIES = {"grid": 0, "line": 1, "total": 2, "tree": 3, "tree2": 3, "tree3": 4, "tree4": 5}
 DISTS = {"constant": 0, "uniform": 1, "exponential": 2}
 KIND_SERVER, KIND_CLIENT, KIND_HOST, KIND_SIM_CLIENT, KIND_SERVICE = 0, 1, 2, 3, 4
@@ -19,6 +19,9 @@ TYPES = dict(init=1, init_ok=2, error=3, echo=10, echo_ok=11, topology=20, topol
              replicate_one=32, replicate_full=33, write=40, write_ok=41, cas=42, cas_ok=43, ts=44, ts_ok=45,
              request_vote=50, request_vote_res=51, append_entries=52, append_entries_res=53,
              txn=60, txn_ok=61)
+# the kafka workload's types (MS_T_SEND ...): the device's own encoding, unknown to the JSON envelope and the oracle
+KAFKA_TYPES = dict(send=70, send_ok=71, poll=72, poll_ok=73, commit_offsets=74, commit_offsets_ok=75,
+                   list_committed_offsets=76, list_committed_offsets_ok=77)
 TYPE_NAMES = {v: k for k, v in TYPES.items()}
 F_MSG_ID, F_REPLY, F_CREATE, F_APPENDS = 1, 2, 4, 8
 RECV_BIT = 1 << 63
@@ -32,7 +35,7 @@ class SimError(RuntimeError):
 
 def body(type, msg_id=None, in_reply_to=None, p0=0, p1=0, create=False, appends=False):
     b = Body()
-    b.type = TYPES[type] if isinstance(type, str) else type
+    b.type = (TYPES[type] if type in TYPES else KAFKA_TYPES[type]) if isinstance(type, str) else type
     b.flags = ((F_MSG_ID if msg_id is not None else 0) | (F_REPLY if in_reply_to is not None else 0) |
                (F_CREATE if create else 0) | (F_APPENDS if appends else 0))
     b.msg_id = msg_id or 0
@@ -95,7 +98,8 @@ class Sim:
             cfg.reserved[3] = SERVICES.index(name) if isinstance(name, str) else int(name)
         # named spellings of ms_config.reserved[]
         for name, slot in (("history_rounds", 0), ("use_graph", 1), ("n_keys", 2), ("raft_log_cap", 3),
-                           ("raft_group", 4), ("rpc_table", 5), ("tree_ptrs", 3), ("tree_cache", 4)):
+                           ("raft_group", 4), ("rpc_table", 5), ("tree_ptrs", 3), ("tree_cache", 4),
+                           ("kafka_keys", 2), ("kafka_log_cap", 3)):
             if name in sizing:
                 cfg.reserved[slot] = int(sizing.pop(name))
         for k, v in sizing.items():
@@ -174,6 +178,41 @@ class Sim:
         g = int(self.cfg.reserved[4])
         self.kv_groups = (first, 2 * (g if 0 < g < self.n_nodes else self.n_nodes))   # first client, clients per group
         return first
+
+    def add_kafka_clients(self, n_clients, interval_ns, time_limit_ns, assign_permille=0, crash_permille=0,
+                          timeout_ns=0, first_name=0):
+        """ms_add_kafka_clients: closed-loop kafka clients of the single-node logs on the device (client k on server
+        k mod n_nodes); returns the first endpoint index.  kafka_history() returns their records; sim.kafka_groups =
+        (first client, servers per group g = raft_group, 0 = 1)"""
+        kc = _lib.KafkaGenConfig(n_clients, assign_permille, crash_permille, 0, interval_ns, timeout_ns, time_limit_ns)
+        first = self._chk(self.L.ms_add_kafka_clients(self.h, C.byref(kc), first_name))
+        self.kafka_groups = (first, max(1, int(self.cfg.reserved[4])))
+        return first
+
+    def kafka_history(self, cap=1 << 20):
+        """ms_kafka_history_drain: the kafka clients' records since the last call, in (time, round, client) order"""
+        parts = []
+        while True:
+            out = np.zeros(cap, dtype=_lib.KAFKA_HIST_DTYPE)
+            n = C.c_size_t(0)
+            self._chk(self.L.ms_kafka_history_drain(self.h, out.ctypes.data, cap, C.byref(n)))
+            parts.append(out[:n.value])
+            if n.value < cap:
+                break
+        return np.concatenate(parts)
+
+    def kafka_log(self, node, key):
+        """ms_kafka_log: the messages of node's log of `key`, offset order"""
+        n = C.c_size_t(0)
+        self._chk(self.L.ms_kafka_log(self.h, node, key, None, 0, C.byref(n)))
+        out = np.zeros(n.value, dtype=np.uint32)
+        self._chk(self.L.ms_kafka_log(self.h, node, key, out.ctypes.data, n.value, C.byref(n)))
+        return out
+
+    def kafka_committed(self, node, key):
+        """ms_kafka_committed: node's committed offset of `key`, None when nothing is committed"""
+        c = self.L.ms_kafka_committed(self.h, node, key)
+        return None if c == -1 else self._chk(c)
 
     def history(self, cap=1 << 20):
         """ms_history_drain: the history records since the last call, in (time, round, client) order"""
@@ -435,6 +474,7 @@ class Sim:
 
 HIST_TYPES = ("invoke", "ok", "fail", "info")              # MS_H_*
 HF_KV_READ, HF_KV_WRITE, HF_KV_CAS = 2, 3, 4              # MS_HF_KV_*
+HF_KAFKA_SEND, HF_KAFKA_POLL, HF_KAFKA_ASSIGN, HF_KAFKA_CRASH = 10, 11, 12, 13   # MS_HF_KAFKA_*
 H_NEMESIS = 0xFFFFFFFF                                    # MS_H_NEMESIS: the client of a nemesis record
 HF_NEM_ONE, HF_NEM_MAJORITY, HF_NEM_MINORITY_THIRD, HF_NEM_STOP = 5, 6, 7, 8   # MS_HF_NEM_*
 HF_NEM_MAJORITIES_RING = 9                                # MS_HF_NEM_MAJORITIES_RING
