@@ -1883,6 +1883,14 @@ __device__ void sv_step(const Params& p, DevState* st, uint32_t e, uint64_t roun
 #ifndef MS_ROUND_MINB2
 #define MS_ROUND_MINB2 4
 #endif
+// window slots a thread has in flight in PA1 (record loads) and PA2 (seen-set words).  PA1 at one slot keeps the
+// loop's invariants in registers; 2 deep spills more and measured 3.5 % slower, 3 and 4 deep slower still (DESIGN 3.5)
+#ifndef MS_PA1_DEPTH
+#define MS_PA1_DEPTH 1
+#endif
+#ifndef MS_PA2_DEPTH
+#define MS_PA2_DEPTH 4
+#endif
 // Default shape of window-size class CLS (ms_engine.cu build_sim: ladder / thr_default).  The FIX instantiations
 // assume it, which turns every shared-memory array base and every loop stride into an immediate; a simulation
 // sized differently (max_window below the ladder, threads_per_node) runs the generic ones.
@@ -2088,7 +2096,7 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     if (nb_smem && tid < (int)deg) s_nbr[tid] = p.nbr[p.nbr_off[e] + tid];
     __syncthreads();
 
-    // PA1: one pass over the window in arrival order, loads 2 records deep: order keys,
+    // PA1: one pass over the window in arrival order, MS_PA1_DEPTH records per thread in flight: order keys,
     //      partition check at dequeue (net.clj:234), compact message class
     {
       uint32_t err_val = 0xFFFFFFFFu;
@@ -2098,15 +2106,15 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       const bool nb4 = nb_smem && deg <= 4;
       const uint32_t nr0 = (nb4 && deg > 0) ? s_nbr[0] : 0xFFFFFFFFu, nr1 = (nb4 && deg > 1) ? s_nbr[1] : 0xFFFFFFFFu;
       const uint32_t nr2 = (nb4 && deg > 2) ? s_nbr[2] : 0xFFFFFFFFu, nr3 = (nb4 && deg > 3) ? s_nbr[3] : 0xFFFFFFFFu;
-      for (int base = 0; base < (int)n; base += 2 * nt) {
-        uint4 a[2], b[2], c[2];
+      for (int base = 0; base < (int)n; base += MS_PA1_DEPTH * nt) {
+        uint4 a[MS_PA1_DEPTH], b[MS_PA1_DEPTH], c[MS_PA1_DEPTH];
 #pragma unroll
-        for (int q = 0; q < 2; q++) {
+        for (int q = 0; q < MS_PA1_DEPTH; q++) {
           const int i = base + q * nt + tid;
           if (i < (int)n) win_load(p, win, e, round, (uint32_t)i, a[q], b[q], c[q]);   // compact slots: one load
         }
 #pragma unroll
-        for (int q = 0; q < 2; q++) {
+        for (int q = 0; q < MS_PA1_DEPTH; q++) {
           const int i = base + q * nt + tid;
           if (i >= (int)n) continue;
           const uint64_t rnd = (uint64_t)a[q].z | ((uint64_t)a[q].w << 32);
@@ -2176,16 +2184,16 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
     }
     // PA2: seen-set test of the broadcast values (own slots only: no barrier needed in between)
     if (bcast) {
-      for (int base = 0; base < (int)n; base += 4 * nt) {
-        uint32_t w[4], vv[4];
+      for (int base = 0; base < (int)n; base += MS_PA2_DEPTH * nt) {
+        uint32_t w[MS_PA2_DEPTH], vv[MS_PA2_DEPTH];
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
+        for (int q = 0; q < MS_PA2_DEPTH; q++) {
           const int i = base + q * nt + tid;
           vv[q] = i < (int)n ? vals[i] : 0u;
           w[q] = (vv[q] & V_CAND) ? mybits[(vv[q] & V_MASK) >> 5] : 0xFFFFFFFFu;
         }
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
+        for (int q = 0; q < MS_PA2_DEPTH; q++) {
           const int i = base + q * nt + tid;
           if (i < (int)n && (vv[q] & V_CAND) && !((w[q] >> (vv[q] & 31)) & 1u)) vals[i] = vv[q] | V_FRESH;
         }
@@ -3133,7 +3141,18 @@ static msk_round_fn msk_round_kernel(uint32_t family, int cls, bool fixed = fals
   return tab[family & 7u][cls];
 }
 
+// Occupancy experiment (tools/occupancy_sweep.py): extra bytes of dynamic shared memory for every class-2 (2048-slot)
+// launch, so that fewer of its CTAs fit on an SM.  0 in the product library.
+#ifndef MS_CLS2_SMEM_PAD
+#define MS_CLS2_SMEM_PAD 0
+#endif
+
+size_t msk_round_smem_bytes(uint32_t cap) {
+  return (size_t)cap * 25 + 32 + (cap == msd::kClsLadder[2] ? (size_t)MS_CLS2_SMEM_PAD : 0);
+}
+
 cudaError_t msk_round_smem_attr(size_t bytes) {
+  if (MS_CLS2_SMEM_PAD && bytes < msk_round_smem_bytes(msd::kClsLadder[2])) bytes = msk_round_smem_bytes(msd::kClsLadder[2]);
   cudaError_t e = cudaSuccess;
   for (uint32_t f = 0; f < 8 && e == cudaSuccess; f++)
     for (int c = 0; c < 4 && e == cudaSuccess; c++)
@@ -3143,8 +3162,6 @@ cudaError_t msk_round_smem_attr(size_t bytes) {
     e = cudaFuncSetAttribute(msk_round_kernel(0, c, true), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
   return e;
 }
-
-size_t msk_round_smem_bytes(uint32_t cap) { return (size_t)cap * 25 + 32; }
 
 void msk_set_bit(uint32_t* words, size_t word, uint32_t bit, cudaStream_t s) {
   MS_LAUNCH(msd::k_set_bit, 1, 1, 0, s, words, word, bit);
