@@ -110,7 +110,11 @@ enum {
    * has len_i messages and [o_i, len_i) is what the poll returns (ms_kafka_log).  commit_offsets_ok: empty.
    * list_committed_offsets p0 = k0 | k1 << 16; its _ok p0 = the keys that are present, p1 = their offsets. */
   MS_T_SEND = 70, MS_T_SEND_OK = 71, MS_T_POLL = 72, MS_T_POLL_OK = 73, MS_T_COMMIT_OFFSETS = 74,
-  MS_T_COMMIT_OFFSETS_OK = 75, MS_T_LIST_COMMITTED_OFFSETS = 76, MS_T_LIST_COMMITTED_OFFSETS_OK = 77
+  MS_T_COMMIT_OFFSETS_OK = 75, MS_T_LIST_COMMITTED_OFFSETS = 76, MS_T_LIST_COMMITTED_OFFSETS_OK = 77,
+  /* g-counter / pn-counter (workload/pn_counter.clj:20-32, demo/ruby/crdt.rb, DESIGN.md 2.16): add = MS_T_ADD with
+   * p0 = delta (int32), add_ok empty; read = MS_T_READ, read_ok p1 = the value (int64).  merge p1 = k: the sender's
+   * k-th run of its replication task, whose {inc, dec} snapshot stays on the device; merge_ok empty */
+  MS_T_MERGE = 80, MS_T_MERGE_OK = 81
 };
 
 enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* --workload, core.clj:36-47 */
@@ -135,7 +139,7 @@ enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* 
                             other request type crashes the node: later messages are received, with no effect, and it
                             never sends again.  A missing service endpoint latches "Invalid dest".  No timers; one GPU.
                             reserved[4] = g groups the servers for ms_add_kv_clients only. */
-       MS_W_KAFKA = 7 };   /* kafka served by single-node logs (demo/clojure/kafka_single_node.clj, DESIGN.md 2.15): every
+       MS_W_KAFKA = 7,     /* kafka served by single-node logs (demo/clojure/kafka_single_node.clj, DESIGN.md 2.15): every
                             node keeps its own append-only log per key, ms_config.reserved[2] keys (0 = 16, <= 65535) of
                             reserved[3] messages each (0 = 4096).  init -> init_ok; send appends and answers offset =
                             count - 1; poll answers every requested key whose log is longer than the offset;
@@ -144,6 +148,18 @@ enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* 
                             A key >= reserved[2] latches E_VALUE_RANGE, an append to a full log a capacity error
                             (MS_ERR_SIM).  reserved[4] = g groups the servers for ms_add_kafka_clients (0 = 1).  No
                             timers; one GPU. */
+       MS_W_G_COUNTER = 8, /* g-counter, and */
+       MS_W_PN_COUNTER = 9 }; /* pn-counter: both run the PN-counter CRDT node (demo/ruby/pn_counter.rb on crdt.rb and
+                            node.rb, DESIGN.md 2.16); the workloads differ only in the clients' deltas.  A node's init node_ids is its block of g = reserved[4] consecutive servers (0 = all servers),
+                            g <= 1024.  State: one inc and one dec entry per block member.  init -> init_ok and (re)starts
+                            the replication task: first run in the next round, then every gset_interval_ms; a run, before
+                            the node's receives, snapshots the state and sends merge (p1 = run) to every other block
+                            member in index order.  add: delta >= 0 adds to inc[self], else -delta to dec[self]; read_ok
+                            p1 = sum inc - sum dec; merge takes the element-wise max with the named snapshot (one that is
+                            not resident, or a merge not sent by a block member's task, latches E_SNAPSHOT), answers
+                            merge_ok; merge_ok does nothing.  Replies carry in_reply_to only when the request had a
+                            msg_id; a message with in_reply_to is ignored.  Any other type crashes the node: later
+                            messages are received, with no effect, and it never sends again.  One GPU. */
 enum { MS_TOPO_GRID = 0, MS_TOPO_LINE = 1, MS_TOPO_TOTAL = 2,                /* --topology, broadcast.clj:169-178 */
        MS_TOPO_TREE2 = 3, MS_TOPO_TREE3 = 4, MS_TOPO_TREE4 = 5 };
 enum { MS_DIST_CONSTANT = 0, MS_DIST_UNIFORM = 1, MS_DIST_EXPONENTIAL = 2 }; /* --latency-dist, net.clj:73-77 */
@@ -180,7 +196,7 @@ typedef struct ms_config {
   uint32_t seed_lo, seed_hi; /* Philox key; the reference is unseeded */
   double   p_loss;           /* net.clj:100 starts at 0; no CLI flag upstream */
   uint32_t n_values;         /* size of the value universe (seen-set bitmap bits per node) */
-  uint32_t gset_interval_ms; /* g-set replication period (demo/ruby/g_set.rb:34) */
+  uint32_t gset_interval_ms; /* CRDT replication period: g-set (demo/ruby/g_set.rb:34), g-counter / pn-counter (crdt.rb) */
   /* engine sizing (0 = default) */
   uint32_t max_endpoints;    /* servers + clients + services */
   uint32_t ring_cap;         /* per-endpoint inbox ring capacity, power of two */
@@ -197,7 +213,7 @@ typedef struct ms_config {
                               * in the size classes of windows up to 2048 */
   uint32_t n_shards;         /* GPUs the endpoints are sharded over (0/1 = single GPU), <= 8 */
   uint32_t shard_id;         /* this process's shard */
-  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn / proxy node (0 = 4096).  MS_W_KV_PROXY: [3] = the backing service MS_SVC_*, [4] = g for ms_add_kv_clients.  MS_W_KAFKA: [2] = keys per node (0 = 16, <= 65535), [3] = log capacity per key (0 = 4096), [4] = g for ms_add_kafka_clients (0 = 1) */
+  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn / proxy node (0 = 4096).  MS_W_KV_PROXY: [3] = the backing service MS_SVC_*, [4] = g for ms_add_kv_clients.  MS_W_KAFKA: [2] = keys per node (0 = 16, <= 65535), [3] = log capacity per key (0 = 4096), [4] = g for ms_add_kafka_clients (0 = 1).  MS_W_G_COUNTER / MS_W_PN_COUNTER: [4] = g, servers per block (0 = all, <= 1024) */
   /* ABI 2.  Servers and the other endpoints (clients, hosts, services) may be sized apart: a
    * service hears from every node, a node from a few.  0 = ring_cap / max_window. */
   uint32_t server_ring_cap;  /* inbox ring capacity of the servers, power of two */
@@ -258,7 +274,13 @@ int     ms_recv_json(ms_sim* sim, uint32_t endpoint, int64_t timeout_virtual_ns,
  * Every invocation and completion is a 32-byte history record; ms_history_drain hands them over in
  * (time, round, client) order -- the Jepsen history a checker (set-full) works on.  A read's value is
  * the node's set at that moment: the record carries its size, the members of a FINAL read are what
- * ms_node_set returns once the run is over (nothing changes after the final reads). */
+ * ms_node_set returns once the run is over (nothing changes after the final reads).
+ * g-counter / pn-counter (MS_W_G_COUNTER / MS_W_PN_COUNTER, DESIGN.md 2.16): the same clients, with the client of
+ * workload/pn_counter.clj:35-53.  Word 0 of the op's draw against read_permille picks a read or an add; the add's
+ * delta is (word 2 * 10 >> 32) - 5 for pn-counter, (word 2 * 5 >> 32) for g-counter; the add's record is
+ * MS_HF_COUNTER_ADD with value = the delta (int32 bits), a read ok's value is the read's (int32 bits; a read_ok
+ * outside int32 latches E_VALUE_RANGE).  The counter client has no with-errors: a time-out or an error reply is :info,
+ * reads included.  The final reads are gen/each-thread {:f :read :final? true} (pn_counter.clj:136). */
 typedef struct ms_gen_config {
   uint32_t n_clients;
   uint32_t read_permille;    /* share of reads in the mix, out of 1000 (gen/mix: 500) */
@@ -278,7 +300,7 @@ typedef struct ms_hist {
   uint32_t value;            /* broadcast / add: the value; read ok: the size of the set returned */
 } ms_hist;
 enum { MS_H_INVOKE = 0, MS_H_OK = 1, MS_H_FAIL = 2, MS_H_INFO = 3, MS_H_TIMEOUT = 0xFFFF };
-enum { MS_HF_BROADCAST = 0, MS_HF_READ = 1 };
+enum { MS_HF_BROADCAST = 0, MS_HF_READ = 1, MS_HF_COUNTER_ADD = 14 };
 /* adds cfg->n_clients endpoints "c<first_name> ..." and returns the index of the first; once per simulation */
 int ms_add_gen_clients(ms_sim* sim, const ms_gen_config* cfg, uint32_t first_name);
 int ms_history_drain(ms_sim* sim, ms_hist* out, size_t cap, size_t* n_out);
@@ -378,6 +400,11 @@ int ms_kafka_history_drain(ms_sim* sim, ms_kafka_hist* out, size_t cap, size_t* 
 int ms_kafka_log(ms_sim* sim, uint32_t node, uint32_t key, uint32_t* msgs, size_t cap, size_t* len);
 /* MS_W_KAFKA: node's committed offset of `key`, -1 when none; MS_ERR_ARG on another workload or a bad node / key */
 int64_t ms_kafka_committed(ms_sim* sim, uint32_t node, uint32_t key);
+
+/* MS_W_G_COUNTER / MS_W_PN_COUNTER: node's counter, one entry per member of its block, inc then dec, in block order.
+ * Copies at most cap entries into out and returns the count 2 x (the block's size); MS_ERR_ARG on another workload or a
+ * bad node */
+int ms_counter_state(ms_sim* sim, uint32_t node, int64_t* out, size_t cap);
 
 /* Upload a time-sorted schedule of client ops (appends). */
 int ms_schedule_ops(ms_sim* sim, const ms_op* ops, size_t n);

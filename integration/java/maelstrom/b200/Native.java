@@ -62,6 +62,7 @@ public final class Native {
   public static native int raftState(long h, int node, ByteBuffer out8);
   public static native long kafkaLog(long h, int node, int key, ByteBuffer msgsU32, long cap);
   public static native long kafkaCommitted(long h, int node, int key);
+  public static native int counterState(long h, int node, ByteBuffer outI64, long cap);
   public static native int counters(long h, ByteBuffer out8);
   public static native int ringCounters(long h, ByteBuffer out, int n);
   public static native int setOrigin(long h, long round, long msgId, long eventId, int ringPos, int ringStride);

@@ -108,6 +108,7 @@ SYMBOLS = {
     "ms_kafka_history_drain": (C.c_int, [_P, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "ms_kafka_log": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "ms_kafka_committed": (C.c_int64, [_P, C.c_uint32, C.c_uint32]),
+    "ms_counter_state": (C.c_int, [_P, C.c_uint32, _P, C.c_size_t]),
     "ms_schedule_ops": (C.c_int, [_P, _P, C.c_size_t]),
     "ms_step": (C.c_int, [_P, C.c_uint64]),
     "ms_run": (C.c_int, [_P, C.c_int64]),

@@ -268,6 +268,13 @@ struct Params {
   struct KfGenDev* kf_gc;    // [max_endpoints], valid where gc is a kafka client's
   uint4*    kf_hist;         // ring of 64-B ms_kafka_hist records
   uint32_t  kf_hist_mask, kf_assign_permille, kf_crash_permille, kf_pad;
+  // MS_W_G_COUNTER / MS_W_PN_COUNTER (ct_handle in csrc/ms_raft.cuh): per node its counter, inc then dec, one entry per
+  // member of its block (ct_width = the block size rf_group, or every server); the replication task's snapshot rows
+  // (row = node * gs_slots + run % gs_slots).  The task's schedule, run numbers and row tags are g-set's gs_init /
+  // gs_next_fire / gs_fires / gs_tag.  Appended
+  int64_t*  ct_val;          // [n_servers][2 * ct_width]
+  int64_t*  ct_snap;         // [n_servers * gs_slots][2 * ct_width]
+  uint32_t  ct_width, ct_pad;
 };
 
 constexpr uint32_t kRaftCallbacks = 4096;       // default pending-RPC table slots per node (ms_config.reserved[5]; oracle: same)

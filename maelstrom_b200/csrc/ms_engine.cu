@@ -96,7 +96,7 @@ static const char* dev_error_text(uint32_t code) {
     case E_RAFT_CAPACITY: return "Raft node out of log / staging / payload-heap capacity (raise ms_config.reserved[3]) at node";
     case E_KAFKA_CAPACITY: return "kafka node's log of a key is full (raise ms_config.reserved[3]) at node";
     case E_HISTORY_RING: return "history ring of the closed-loop clients is full (call ms_history_drain more often) at client";
-    case E_SNAPSHOT: return "replicate_full names a set snapshot that is not resident (in flight longer than calendar_slots, or forged): sender";
+    case E_SNAPSHOT: return "replicate_full names a set snapshot that is not resident (in flight longer than calendar_slots, or forged), or a merge a counter snapshot that is not: sender";
   }
   return "unknown device error";
 }
@@ -596,11 +596,21 @@ struct ms_sim {
   }
 };
 
+// Rotating snapshot rows per node for a CRDT replication task (g-set's replicate_full, the counters' merge): a
+// snapshot stays resident while its messages can be in flight, i.e. at most calendar_slots ticks, with one run every
+// gset_interval_ms.  (The exponential law is unbounded: 48 means = a tail of e^-48; beyond that, e.g. after slow!, a
+// message that outlives its snapshot row is reported as E_SNAPSHOT.)
+static uint32_t snapshot_slots(const ms_config& c, bool use_calendar) {
+  const uint32_t span_ms = !use_calendar ? 0u
+      : std::max<uint32_t>(c.calendar_slots, c.latency_dist == MS_DIST_EXPONENTIAL ? 48u * c.latency_mean_ms : 2u * c.latency_mean_ms);
+  return std::min<uint32_t>(pow2_at_least(span_ms / c.gset_interval_ms + 2u), 1024u);
+}
+
 static int build_sim(ms_sim* s, const ms_config* in) {
   ms_config& c = s->cfg;
   c = *in;
   if (c.n_nodes == 0) { set_err("n_nodes must be positive (--node-count)"); return MS_ERR_ARG; }
-  if (c.workload > MS_W_KAFKA || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
+  if (c.workload > MS_W_PN_COUNTER || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
     set_err("bad workload/topology/latency_dist");
     return MS_ERR_ARG;
   }
@@ -815,6 +825,28 @@ static int build_sim(ms_sim* s, const ms_config* in) {
     CK(cudaMemsetAsync(P.kf_committed, 0xFF, N * P.kf_keys * 4, s->stream));   // kKafkaAbsent: nothing committed
     CK(cudaStreamSynchronize(s->stream));
   }
+  if (c.workload == MS_W_G_COUNTER || c.workload == MS_W_PN_COUNTER) {
+    // counter nodes (ct_handle, csrc/ms_raft.cuh): per node its counter and the replication task's snapshot rows, sized
+    // and scheduled as g-set's; the staging rows of the sequential step (a run's merges, then one reply per message)
+    if (c.n_shards > 1) { set_err("MS_W_G_COUNTER / MS_W_PN_COUNTER run on one GPU"); return MS_ERR_ARG; }
+    const uint32_t g = c.reserved[4] && c.reserved[4] < c.n_nodes ? c.reserved[4] : c.n_nodes;
+    if (g > 1024u) {
+      set_err("MS_W_G_COUNTER / MS_W_PN_COUNTER: at most 1024 servers per block (ms_config.reserved[4], 0 = all servers)");
+      return MS_ERR_ARG;
+    }
+    const size_t N = c.n_nodes;
+    P.rf_group = g < c.n_nodes ? g : 0u;
+    P.ct_width = g;
+    P.rf_stage_cap = c.server_max_window + g + 16u;
+    P.rf_cb_mask = 0;
+    P.gs_interval_ms = c.gset_interval_ms;
+    P.gs_slots = snapshot_slots(c, s->use_calendar);
+    const size_t rows = N * P.gs_slots;
+    if ((rc = s->dalloc(&P.rf_node, N)) || (rc = s->dalloc(&P.rf_cb, N * 2)) || (rc = s->dalloc(&P.rf_stage, N * P.rf_stage_cap * 3)) ||
+        (rc = s->dalloc(&P.gs_init, N)) || (rc = s->dalloc(&P.gs_next_fire, N)) || (rc = s->dalloc(&P.gs_fires, N)) ||
+        (rc = s->dalloc(&P.gs_tag, rows)) || (rc = s->dalloc(&P.ct_val, N * 2 * g)) || (rc = s->dalloc(&P.ct_snap, rows * 2 * g)))
+      return rc;
+  }
   if (c.workload == MS_W_TXN || c.workload == MS_W_TXN_TREE || c.workload == MS_W_KV_PROXY) {
     // txn-list-append nodes and lin-kv proxies: message ids, the table of pending RPC closures and the staging rows
     // of the sequential step (csrc/ms_raft.cuh); a proxy sends at most once per message it receives
@@ -870,11 +902,7 @@ static int build_sim(ms_sim* s, const ms_config* in) {
     // replicate_full payloads: a snapshot stays resident while its messages can be in flight,
     // i.e. at most calendar_slots ticks; one run every gset_interval_ms (g_set.rb:34)
     P.gs_interval_ms = c.gset_interval_ms;
-    // (the exponential law is unbounded: 48 means = a tail of e^-48; beyond that, e.g. after slow!, a
-    // replicate_full that outlives its snapshot row is reported as E_SNAPSHOT)
-    const uint32_t span_ms = !s->use_calendar ? 0u
-        : std::max<uint32_t>(c.calendar_slots, c.latency_dist == MS_DIST_EXPONENTIAL ? 48u * c.latency_mean_ms : 2u * c.latency_mean_ms);
-    P.gs_slots = std::min<uint32_t>(pow2_at_least(span_ms / c.gset_interval_ms + 2u), 1024u);
+    P.gs_slots = snapshot_slots(c, s->use_calendar);
     const size_t rows = (size_t)c.n_nodes * P.gs_slots;
     if ((rc = s->dalloc(&P.gs_init, c.n_nodes))) return rc;
     if ((rc = s->dalloc(&P.gs_next_fire, c.n_nodes))) return rc;
@@ -1114,8 +1142,9 @@ int ms_add_gen_clients(ms_sim* s, const ms_gen_config* gc, uint32_t first_name) 
   cudaSetDevice(s->device);
   if (!gc || gc->n_clients == 0 || gc->interval_ns <= 0 || gc->read_permille > 1000) { set_err("ms_add_gen_clients: bad configuration"); return MS_ERR_ARG; }
   if (s->P.gc) { set_err("ms_add_gen_clients: the generator's clients exist already"); return MS_ERR_ARG; }
-  if (s->cfg.workload != MS_W_BROADCAST && s->cfg.workload != MS_W_GSET) {
-    set_err("ms_add_gen_clients: the device generator drives the broadcast and g-set workloads");
+  if (s->cfg.workload != MS_W_BROADCAST && s->cfg.workload != MS_W_GSET && s->cfg.workload != MS_W_G_COUNTER &&
+      s->cfg.workload != MS_W_PN_COUNTER) {
+    set_err("ms_add_gen_clients: the device generator drives the broadcast, g-set, g-counter and pn-counter workloads");
     return MS_ERR_ARG;
   }
   if (s->P.n_shards > 1) { set_err("ms_add_gen_clients: single GPU only"); return MS_ERR_ARG; }
@@ -1334,6 +1363,21 @@ int64_t ms_kafka_committed(ms_sim* s, uint32_t node, uint32_t key) {
   CK(cudaStreamSynchronize(s->stream));
   CK(cudaMemcpy(&c, s->P.kf_committed + (size_t)node * s->P.kf_keys + key, 4, cudaMemcpyDeviceToHost));
   return c == kKafkaAbsent ? -1 : (int64_t)c;
+}
+
+int ms_counter_state(ms_sim* s, uint32_t node, int64_t* out, size_t cap) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  if ((s->cfg.workload != MS_W_G_COUNTER && s->cfg.workload != MS_W_PN_COUNTER) || node >= s->cfg.n_nodes) {
+    set_err("ms_counter_state: not a counter node (MS_W_G_COUNTER / MS_W_PN_COUNTER, node < n_nodes)");
+    return MS_ERR_ARG;
+  }
+  const uint32_t W = s->P.ct_width, gbase = node / W * W, gn = std::min(W, s->cfg.n_nodes - gbase);
+  std::vector<int64_t> row(2 * (size_t)W);
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(row.data(), s->P.ct_val + (size_t)node * 2 * W, row.size() * 8, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; out && i < std::min<size_t>(cap, 2 * (size_t)gn); i++) out[i] = row[i < gn ? i : W + i - gn];
+  return (int)(2 * gn);
 }
 
 int ms_history_drain(ms_sim* s, ms_hist* out, size_t cap, size_t* n_out) {
@@ -1798,7 +1842,9 @@ int ms_set_nemesis(ms_sim* s, const ms_nemesis_config* nc) {
   if (s->cfg.reserved[1] == 1) { set_err("ms_set_nemesis: not with CUDA-graph replay (ms_config.reserved[1] = 1)"); return MS_ERR_ARG; }
   if (s->np.comp_active) { set_err("ms_set_nemesis: a bulk partition is installed (ms_net_heal first)"); return MS_ERR_ARG; }
   const uint32_t N = s->cfg.n_nodes;
-  const uint32_t natural = (s->cfg.workload == MS_W_RAFT && P.rf_group) ? P.rf_group : N;
+  // Raft clusters and counter blocks are closed under the nodes' traffic
+  const bool blocks = s->cfg.workload == MS_W_RAFT || s->cfg.workload == MS_W_G_COUNTER || s->cfg.workload == MS_W_PN_COUNTER;
+  const uint32_t natural = (blocks && P.rf_group) ? P.rf_group : N;
   const uint32_t gsz = nc->group ? nc->group : natural;
   if (gsz != natural || gsz == 0 || gsz > kNemMaxGroup) {
     set_err("ms_set_nemesis: bad group (the workload's clusters have " + std::to_string(natural) +
@@ -2215,7 +2261,7 @@ uint64_t ms_undeliverable(ms_sim* s) { std::lock_guard<std::mutex> g(s->mu); ret
 int ms_raft_state(ms_sim* s, uint32_t node, uint64_t out[8]) {
   std::lock_guard<std::mutex> g(s->mu);
   cudaSetDevice(s->device);
-  if (!s->P.rf_node || node >= s->cfg.n_nodes || s->cfg.workload == MS_W_KAFKA) { set_err("ms_raft_state: not a Raft node"); return MS_ERR_ARG; }
+  if (!s->P.rf_node || node >= s->cfg.n_nodes || s->cfg.workload >= MS_W_KAFKA) { set_err("ms_raft_state: not a Raft node"); return MS_ERR_ARG; }
   RaftDev r;
   CK(cudaStreamSynchronize(s->stream));
   CK(cudaMemcpy(&r, s->P.rf_node + node, sizeof r, cudaMemcpyDeviceToHost));

@@ -223,6 +223,12 @@ jlong FN(kafkaLog)(JNIEnv* env, jclass c, jlong h, jint node, jint key, jobject 
   return rc < 0 ? (jlong)rc : (jlong)n;
 }
 jlong FN(kafkaCommitted)(JNIEnv* env, jclass c, jlong h, jint node, jint key) { (void)env; (void)c; return ms_kafka_committed(H(h), (uint32_t)node, (uint32_t)key); }
+/* the counter of a g-counter / pn-counter node: out = direct buffer of cap i64 (inc then dec); returns 2 x its block's
+ * size or a negative error */
+jint FN(counterState)(JNIEnv* env, jclass c, jlong h, jint node, jobject out, jlong cap) {
+  (void)c;
+  return ms_counter_state(H(h), (uint32_t)node, out ? (int64_t*)BUF(out) : NULL, (size_t)cap);
+}
 jint FN(counters)(JNIEnv* env, jclass c, jlong h, jobject out8) { (void)c; return ms_counters(H(h), (uint64_t*)BUF(out8)); }
 /* out = direct buffer of n u64 (>= 6 x n_nodes): tail / limit / head of the 48-B rings, then of the compact rings */
 jint FN(ringCounters)(JNIEnv* env, jclass c, jlong h, jobject out, jint n) { (void)c; return ms_ring_counters(H(h), (uint64_t*)BUF(out), (uint32_t)n); }

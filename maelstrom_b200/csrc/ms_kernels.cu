@@ -758,6 +758,72 @@ __device__ bool kf_gen_step(const Params& p, DevState* st, uint32_t e, int64_t n
   return send;
 }
 
+// The g-counter / pn-counter client (ms_add_gen_clients on MS_W_G_COUNTER / MS_W_PN_COUNTER, DESIGN.md 2.16): gen_step's
+// phases, quiet period and final read, with the client of workload/pn_counter.clj:35-53 and its generator (:133-136,
+// g_counter.clj:30-40); the oracle's twin is tests/native/counter_oracle.cpp.  The client has no with-errors, so every
+// time-out or error completes as :info, reads included.  GenDev keeps gen_step's meaning: gen_timer_due and gen_wake_ns
+// hold for it as they are.
+__device__ bool ct_gen_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const uint4* myring,
+                            uint32_t head, uint32_t my_mask, uint32_t n, const uint16_t* ord, const uint32_t* vals, Rec& out) {
+  GenDev g = p.gc[e];
+  for (uint32_t pos = 0; pos < n; pos++) {
+    const uint32_t i = ord[pos];
+    if (!(vals[i] & (1u << 30))) continue;                                 // V_RECV: cut by a partition
+    const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
+    const uint4 vb = rp[1], vc = rp[2];
+    const uint32_t type = vc.x & 0xFFFFu, flags = vc.x >> 16;
+    if (!g.waiting_for || !(flags & MS_F_REPLY) || vb.w != g.waiting_for) continue;   // client.clj:106-107
+    uint32_t outcome = MS_H_OK, err = 0, value = g.cur_value;
+    if (type == MS_T_ERROR) {
+      err = vc.y;
+      outcome = MS_H_INFO;
+    } else if (g.cur_f == MS_HF_READ) {                                    // read_ok: (long value), kept as int32
+      const int64_t v = (int64_t)((uint64_t)vc.z | ((uint64_t)vc.w << 32));
+      if (v != (int64_t)(int32_t)v) latch_error(st, E_VALUE_RANGE, e);
+      value = (uint32_t)v;
+    }
+    gen_hist(p, st, now, round, e, g, g.ops, outcome, g.cur_f, err, value);
+    g.waiting_for = 0;
+  }
+  if (g.waiting_for && now >= g.deadline_ns) {                             // client.clj:96-101
+    gen_hist(p, st, now, round, e, g, g.ops, MS_H_INFO, g.cur_f, MS_H_TIMEOUT, g.cur_value);
+    g.waiting_for = 0;
+  }
+  bool send = false;
+  if (!g.waiting_for) {
+    uint32_t f = MS_HF_READ, value = 0;
+    if (g.phase == GEN_MIX) {
+      if (now >= p.gc_limit_ns) g.phase = GEN_QUIET;
+      else if (now >= g.next_op_ns) {
+        uint32_t x[4];
+        philox4x32_10(g.ops, e, 0xC11E47u, 0u, p.seed_lo, p.seed_hi, x);   // the client's own stream: op k
+        if ((((uint64_t)x[0] * 1000u) >> 32) >= p.gc_read_permille) {
+          f = MS_HF_COUNTER_ADD;                                           // (- (rand-int 10) 5), or g-counter's 0..4
+          value = p.workload == MS_W_PN_COUNTER ? (uint32_t)((int32_t)(((uint64_t)x[2] * 10u) >> 32) - 5)
+                                                : (uint32_t)(((uint64_t)x[2] * 5u) >> 32);
+        }
+        g.next_op_ns = now + (int64_t)(((unsigned __int128)x[1] * (unsigned __int128)(2 * (uint64_t)p.gc_interval_ns)) >> 32);
+        send = true;
+      }
+    }
+    if (g.phase == GEN_QUIET && now >= p.gc_limit_ns + p.gc_quiet_ns) { g.phase = GEN_FINAL; send = true; }   // :136
+    else if (g.phase == GEN_FINAL && !send) g.phase = GEN_DONE;
+    if (send) {
+      g.ops++;
+      g.cur_f = f; g.cur_value = value;
+      g.waiting_for = ++g.next_msg_id;                                     // client.clj:61-64
+      g.deadline_ns = now + p.gc_timeout_ns;
+      gen_hist(p, st, now, round, e, g, g.ops, MS_H_INVOKE, f, 0, value);
+      out.round = 0; out.ticket = 0; out.idx = 0;
+      out.src = e; out.dest = g.node; out.msg_id = g.waiting_for; out.in_reply_to = 0;
+      out.tf = (f == MS_HF_READ ? (uint32_t)MS_T_READ : (uint32_t)MS_T_ADD) | ((uint32_t)MS_F_MSG_ID << 16);
+      out.p0 = value; out.p1 = 0;
+    }
+  }
+  p.gc[e] = g;
+  return send;
+}
+
 #include "ms_tree.h"
 #include "ms_raft.cuh"
 
@@ -871,10 +937,11 @@ __device__ void snapshot_endpoints(const Params& p, DevState* st, uint32_t gid, 
       n += cl - ch;
     }
     if (p.kind[e] & kRemoved) n = 0;
-    // g-set: a node whose periodic replication task is due emits even with an empty window
+    // g-set, g-counter / pn-counter: a node whose periodic replication task is due emits even with an empty window
     // Raft: a node whose election / step-down / replication timers are due acts on an empty window too
     const bool timer_due = e < p.n_servers && p.kind[e] == MS_KIND_SERVER &&
                            ((p.workload == MS_W_GSET && p.gs_init[e] && st->now >= p.gs_next_fire[e]) ||
+                            (p.workload >= MS_W_G_COUNTER && p.gs_init[e] && st->now >= p.gs_next_fire[e]) ||
                             (p.workload == MS_W_RAFT && rf_timer_due(p.rf_node[e], st->now)) ||
                             (p.workload == MS_W_TXN_TREE && tt_timer_due(p.tt_node[e], st->now)));
     const bool gen_due = p.gc && p.kind[e] == MS_KIND_GEN_CLIENT && gen_timer_due(p, p.gc[e], st->now);
@@ -938,6 +1005,7 @@ __global__ void k_wake(Params p) {
     // snapshot_endpoints' timer_due / gen_due
     if (e < p.n_servers && p.kind[e] == MS_KIND_SERVER) {
       if (p.workload == MS_W_GSET && p.gs_init[e]) w = min(w, p.gs_next_fire[e]);
+      if (p.workload >= MS_W_G_COUNTER && p.gs_init[e]) w = min(w, p.gs_next_fire[e]);
       if (p.workload == MS_W_RAFT) w = min(w, rf_wake_ns(p.rf_node[e]));
       if (p.workload == MS_W_TXN_TREE) w = min(w, tt_wake_ns(p.tt_node[e]));
     }
@@ -1788,13 +1856,14 @@ __device__ void service_handle(const Params& p, uint32_t svc, const SvReq& q, ui
 }
 
 // ------------------------------------------------------------------ node programs run by k_round
-// Raft / txn-list-append / proxy / kafka server e (ms_raft.cuh), one thread: the window in id order, then the node's timers.
+// Raft / txn-list-append / proxy / kafka / counter server e (ms_raft.cuh), one thread: the window in id order, then the node's timers.
 // Returns the number of sends it staged in rf_stage; k_round emits them.
 __device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const Win& w,
                               uint32_t n, const RoundSmem& sm) {
   RaftCtx c{p, st, e, now, round, p.rf_node + e, p.rf_log + (size_t)e * p.rf_log_cap * 2,
             p.rf_cb + (size_t)e * (p.rf_cb_mask + 1u) * 2, p.rf_stage + (size_t)e * p.rf_stage_cap * 3, 0u, 0u, 0u, 0u};
   rf_group_of(p, e, c.gbase, c.gn);
+  if (p.workload >= MS_W_G_COUNTER) ct_task(c);                  // the counter's replication task: before its receives
   for (uint32_t pos = 0; pos < n; pos++) {
     const uint32_t i = sm.ord[pos];
     if (!(sm.vals[i] & V_RECV)) continue;
@@ -1803,6 +1872,7 @@ __device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t
     else if (p.workload == MS_W_TXN_TREE) tt_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else if (p.workload == MS_W_KV_PROXY) kp_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else if (p.workload == MS_W_KAFKA) kf_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+    else if (p.workload >= MS_W_G_COUNTER) ct_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else txn_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
   }
   if (p.workload == MS_W_RAFT) { rf_actions(c); rf_note_busy(c); }
@@ -2394,10 +2464,11 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       if (tid == 0) {
         Rec q;
         bool send;
-        // the Raft family's clients are the lin-kv ones (ms_add_kv_clients) or the kafka ones (ms_add_kafka_clients);
-        // their requests carry a p1
+        // the Raft family's clients are the lin-kv ones (ms_add_kv_clients), the kafka ones (ms_add_kafka_clients) or
+        // the counter ones (ms_add_gen_clients); their requests carry a p1
         if constexpr (RF) send = p.workload == MS_W_KAFKA ? kf_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q)
-                                                          : kv_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
+                               : p.workload >= MS_W_G_COUNTER ? ct_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q)
+                                                              : kv_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
         else send = gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
         if (send) {
           s_gen[0] = make_uint4(q.src, q.dest, q.msg_id, q.in_reply_to);

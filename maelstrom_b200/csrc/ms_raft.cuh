@@ -604,6 +604,89 @@ __device__ void kf_handle(RaftCtx& c, const Rec& m) {
   rf_emit(c, a);
 }
 
+// ------------------------------------------------------------------ g-counter / pn-counter
+// demo/ruby/pn_counter.rb on crdt.rb and node.rb (DESIGN.md 2.16), for both workloads.  The PN counter is two
+// G-counters, maps node id -> count; a node only ever names the members of its block (node_ids of its init), so the maps
+// are rows of Params.ct_val in block order: inc[0, gn) then dec at + ct_width.  Handlers run in dequeue order, a legal
+// schedule of Ruby's thread per message.  RaftDev.state = 1: crashed (main! raised on a type without a handler).  The
+// replication task keeps g-set's schedule (gs_init / gs_next_fire / gs_fires) and tags its snapshot rows in gs_tag.
+__device__ __forceinline__ int64_t* ct_row(const Params& p, uint32_t e) { return p.ct_val + (size_t)e * 2 * p.ct_width; }
+
+// `every 5` (crdt.rb:41-45, node.rb:129-137), at the start of the node's step: snapshot @value for run k, then
+// merge to every other block member in index order
+__device__ void ct_task(RaftCtx& c) {
+  const Params& p = c.p;
+  if (c.r->state || !p.gs_init[c.e] || c.now < p.gs_next_fire[c.e]) return;
+  const uint32_t k = ++p.gs_fires[c.e];
+  const size_t row = (size_t)c.e * p.gs_slots + (k & (p.gs_slots - 1u));
+  const int64_t* mine = ct_row(p, c.e);
+  int64_t* snap = p.ct_snap + row * 2 * p.ct_width;
+  for (uint32_t i = 0; i < c.gn; i++) { snap[i] = mine[i]; snap[p.ct_width + i] = mine[p.ct_width + i]; }
+  p.gs_tag[row] = k;
+  for (uint32_t n = c.gbase; n < c.gbase + c.gn; n++) {
+    if (n == c.e) continue;
+    Rec m;                                                                        // send! (node.rb:68-78): no msg_id
+    m.round = 0; m.ticket = 0; m.idx = 0;
+    m.src = c.e; m.dest = n; m.msg_id = 0; m.in_reply_to = 0;
+    m.tf = MS_T_MERGE; m.p0 = 0; m.p1 = k;
+    rf_emit(c, m);
+  }
+  p.gs_next_fire[c.e] += (int64_t)p.gs_interval_ms * kTickNs;
+}
+
+__device__ void ct_handle(RaftCtx& c, const Rec& m) {
+  const Params& p = c.p;
+  if (c.r->state) return;                                                         // crashed: read, never acted on
+  const uint32_t type = m.tf & 0xFFFFu, flags = m.tf >> 16;
+  if (flags & MS_F_REPLY) return;                                                 // no callbacks (node.rb:159-164)
+  if (type == MS_T_MERGE_OK) return;                                              // crdt.rb:36-38
+  const bool has_id = (flags & MS_F_MSG_ID) != 0;
+  Rec a;                                                                          // reply! (node.rb:88-91)
+  a.round = 0; a.ticket = 0; a.idx = 0;
+  a.src = c.e; a.dest = m.src; a.msg_id = 0;
+  a.in_reply_to = has_id ? m.msg_id : 0u;                                         // in_reply_to: nil without a msg_id
+  a.p0 = 0; a.p1 = 0;
+  int64_t* mine = ct_row(p, c.e);
+  const uint32_t W = p.ct_width;
+  uint32_t out_type;
+  if (type == MS_T_INIT) {                                                        // node.rb:22-36: (re)starts the task,
+    p.gs_init[c.e] = 1;                                                           // first run in the next round
+    p.gs_next_fire[c.e] = c.now;
+    out_type = MS_T_INIT_OK;
+  } else if (type == MS_T_ADD) {                                                  // pn_counter.rb:77-83
+    const int32_t delta = (int32_t)m.p0;
+    if (delta >= 0) mine[c.e - c.gbase] += delta;
+    else mine[W + c.e - c.gbase] += -(int64_t)delta;
+    out_type = MS_T_ADD_OK;
+  } else if (type == MS_T_READ) {                                                 // crdt.rb:25-27, pn_counter.rb:71-73
+    int64_t v = 0;
+    for (uint32_t i = 0; i < c.gn; i++) v += mine[i] - mine[W + i];
+    a.p1 = (uint64_t)v;
+    out_type = MS_T_READ_OK;
+  } else if (type == MS_T_MERGE) {                                                // crdt.rb:30-34: merge by max
+    const uint32_t k = (uint32_t)m.p1;
+    const size_t row = (size_t)m.src * p.gs_slots + (k & (p.gs_slots - 1u));
+    // only a block member's task sends merges, with its run k >= 1; the row must still hold that run
+    if (m.src < c.gbase || m.src >= c.gbase + c.gn || m.src == c.e || k == 0 || (uint64_t)k != m.p1 ||
+        __ldcg(p.gs_tag + row) != k) {
+      latch_error(c.st, E_SNAPSHOT, m.src);
+      return;
+    }
+    const int64_t* snap = p.ct_snap + row * 2 * W;
+    for (uint32_t i = 0; i < c.gn; i++) {
+      mine[i] = max(mine[i], snap[i]);
+      mine[W + i] = max(mine[W + i], snap[W + i]);
+    }
+    out_type = MS_T_MERGE_OK;
+  } else {
+    c.r->state = 1;                                                               // "No handler": main! raises (node.rb:167),
+    p.gs_init[c.e] = 0;                                                           // the process and its task end
+    return;
+  }
+  a.tf = out_type | ((has_id ? (uint32_t)MS_F_REPLY : 0u) << 16);
+  rf_emit(c, a);
+}
+
 // ------------------------------------------------------------------ txn-list-append on a persistent hash tree
 // demo/ruby/datomic_list_append.rb.  The database is a tree of immutable nodes stored in lww-kv under
 // unique pointers; lin-kv holds the pointer to the root (key "root" = key 0 here).  A txn (:340-353, under

@@ -9,7 +9,7 @@ from . import _lib
 from ._lib import Body, Config, EVENT_DTYPE, JBODY_DTYPE, MSG_DTYPE, OP_DTYPE  # noqa: F401
 
 WORKLOADS = {"echo": 0, "broadcast": 1, "g-set": 2, "lin-kv": 3, "txn-list-append": 4, "txn-list-append-tree": 5,
-             "lin-kv-proxy": 6, "kafka": 7}
+             "lin-kv-proxy": 6, "kafka": 7, "g-counter": 8, "pn-counter": 9}
 TOPOLOGIES = {"grid": 0, "line": 1, "total": 2, "tree": 3, "tree2": 3, "tree3": 4, "tree4": 5}
 DISTS = {"constant": 0, "uniform": 1, "exponential": 2}
 KIND_SERVER, KIND_CLIENT, KIND_HOST, KIND_SIM_CLIENT, KIND_SERVICE = 0, 1, 2, 3, 4
@@ -22,6 +22,8 @@ TYPES = dict(init=1, init_ok=2, error=3, echo=10, echo_ok=11, topology=20, topol
 # the kafka workload's types (MS_T_SEND ...): the device's own encoding, unknown to the JSON envelope and the oracle
 KAFKA_TYPES = dict(send=70, send_ok=71, poll=72, poll_ok=73, commit_offsets=74, commit_offsets_ok=75,
                    list_committed_offsets=76, list_committed_offsets_ok=77)
+# the counter workloads' merge / merge_ok (MS_T_MERGE ...): the device's own encoding, as kafka's
+COUNTER_TYPES = dict(merge=80, merge_ok=81)
 TYPE_NAMES = {v: k for k, v in TYPES.items()}
 F_MSG_ID, F_REPLY, F_CREATE, F_APPENDS = 1, 2, 4, 8
 RECV_BIT = 1 << 63
@@ -35,7 +37,7 @@ class SimError(RuntimeError):
 
 def body(type, msg_id=None, in_reply_to=None, p0=0, p1=0, create=False, appends=False):
     b = Body()
-    b.type = (TYPES[type] if type in TYPES else KAFKA_TYPES[type]) if isinstance(type, str) else type
+    b.type = {**TYPES, **KAFKA_TYPES, **COUNTER_TYPES}[type] if isinstance(type, str) else type
     b.flags = ((F_MSG_ID if msg_id is not None else 0) | (F_REPLY if in_reply_to is not None else 0) |
                (F_CREATE if create else 0) | (F_APPENDS if appends else 0))
     b.msg_id = msg_id or 0
@@ -161,9 +163,12 @@ class Sim:
             self._chk(rc)
             return out[0] if rc == 1 else None
 
-    def add_gen_clients(self, n_clients, interval_ns, time_limit_ns, read_permille=500, timeout_ns=0, quiet_ns=0,
+    def add_gen_clients(self, n_clients, interval_ns, time_limit_ns, read_permille=None, timeout_ns=0, quiet_ns=0,
                         first_name=0):
-        """ms_add_gen_clients: closed-loop clients on the device; returns the first endpoint index"""
+        """ms_add_gen_clients: closed-loop clients on the device; returns the first endpoint index.  read_permille
+        defaults to gen/mix's 500, and to 667 on g-counter, whose gen/filter redraws the negative adds"""
+        if read_permille is None:
+            read_permille = 667 if self.cfg.workload == WORKLOADS["g-counter"] else 500
         gc = _lib.GenConfig(n_clients, read_permille, interval_ns, timeout_ns, time_limit_ns, quiet_ns)
         return self._chk(self.L.ms_add_gen_clients(self.h, C.byref(gc), first_name))
 
@@ -213,6 +218,13 @@ class Sim:
         """ms_kafka_committed: node's committed offset of `key`, None when nothing is committed"""
         c = self.L.ms_kafka_committed(self.h, node, key)
         return None if c == -1 else self._chk(c)
+
+    def counter_state(self, node):
+        """ms_counter_state: node's counter as (inc, dec), int64 arrays with one entry per member of its block"""
+        n = self._chk(self.L.ms_counter_state(self.h, node, None, 0))
+        out = np.zeros(n, dtype=np.int64)
+        self._chk(self.L.ms_counter_state(self.h, node, out.ctypes.data, n))
+        return out[:n // 2], out[n // 2:]
 
     def history(self, cap=1 << 20):
         """ms_history_drain: the history records since the last call, in (time, round, client) order"""
@@ -475,6 +487,7 @@ class Sim:
 HIST_TYPES = ("invoke", "ok", "fail", "info")              # MS_H_*
 HF_KV_READ, HF_KV_WRITE, HF_KV_CAS = 2, 3, 4              # MS_HF_KV_*
 HF_KAFKA_SEND, HF_KAFKA_POLL, HF_KAFKA_ASSIGN, HF_KAFKA_CRASH = 10, 11, 12, 13   # MS_HF_KAFKA_*
+HF_COUNTER_ADD = 14                                       # MS_HF_COUNTER_ADD
 H_NEMESIS = 0xFFFFFFFF                                    # MS_H_NEMESIS: the client of a nemesis record
 HF_NEM_ONE, HF_NEM_MAJORITY, HF_NEM_MINORITY_THIRD, HF_NEM_STOP = 5, 6, 7, 8   # MS_HF_NEM_*
 HF_NEM_MAJORITIES_RING = 9                                # MS_HF_NEM_MAJORITIES_RING
