@@ -114,7 +114,12 @@ enum {
   /* g-counter / pn-counter (workload/pn_counter.clj:20-32, demo/ruby/crdt.rb, DESIGN.md 2.16): add = MS_T_ADD with
    * p0 = delta (int32), add_ok empty; read = MS_T_READ, read_ok p1 = the value (int64).  merge p1 = k: the sender's
    * k-th run of its replication task, whose {inc, dec} snapshot stays on the device; merge_ok empty */
-  MS_T_MERGE = 80, MS_T_MERGE_OK = 81
+  MS_T_MERGE = 80, MS_T_MERGE_OK = 81,
+  /* txn-rw-register (MS_W_TXN_RW, DESIGN.md 2.17): txn = MS_T_TXN with p1 = up to four micro-ops of 16 bits,
+   * valid << 15 | write << 14 | key, and p0 = base: micro-op i, a write, writes base + i (0 = nil); txn_ok = MS_T_TXN_OK
+   * with p0 = the txn's index in the node's log, p1 = its lamport (the read values are in ms_txn_rw_log).  replicate /
+   * replicate_ack p0 = the number of txn+s in the body */
+  MS_T_REPLICATE = 90, MS_T_REPLICATE_ACK = 91
 };
 
 enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* --workload, core.clj:36-47 */
@@ -149,7 +154,7 @@ enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* 
                             (MS_ERR_SIM).  reserved[4] = g groups the servers for ms_add_kafka_clients (0 = 1).  No
                             timers; one GPU. */
        MS_W_G_COUNTER = 8, /* g-counter, and */
-       MS_W_PN_COUNTER = 9 }; /* pn-counter: both run the PN-counter CRDT node (demo/ruby/pn_counter.rb on crdt.rb and
+       MS_W_PN_COUNTER = 9,   /* pn-counter: both run the PN-counter CRDT node (demo/ruby/pn_counter.rb on crdt.rb and
                             node.rb, DESIGN.md 2.16); the workloads differ only in the clients' deltas.  A node's init node_ids is its block of g = reserved[4] consecutive servers (0 = all servers),
                             g <= 1024.  State: one inc and one dec entry per block member.  init -> init_ok and (re)starts
                             the replication task: first run in the next round, then every gset_interval_ms; a run, before
@@ -160,6 +165,21 @@ enum { MS_W_ECHO = 0, MS_W_BROADCAST = 1, MS_W_GSET = 2,                     /* 
                             merge_ok; merge_ok does nothing.  Replies carry in_reply_to only when the request had a
                             msg_id; a message with in_reply_to is ignored.  Any other type crashes the node: later
                             messages are received, with no effect, and it never sends again.  One GPU. */
+       MS_W_TXN_RW = 10 }; /* txn-rw-register served by demo/clojure/txn_rw_register_hat.clj on node.clj (DESIGN.md 2.17).
+                            node.clj parses a replicate's txn+s with string keys, so a replica applies each as an empty
+                            txn (lamport += 1), learns no write and acks with nil timestamps that remove nothing: every
+                            node is an independent serial register store.  A node's init node_ids is its block of g =
+                            reserved[4] consecutive servers (0 = all servers), 2 <= g <= 32.  State: lamport, reserved[2]
+                            keys (0 = 1024, <= 16384; a key >= K latches E_VALUE_RANGE) of {value, lamport}, and the log
+                            of its completed txns, reserved[3] entries (0 = 4096; a full log latches a capacity error).
+                            txn: ts = lamport, lamport += 1, the micro-ops in order (a read returns the value, 0 = nil; a
+                            write overwrites), logged, txn_ok.  The replication task runs every gset_interval_ms (0 = 100)
+                            from the start, before the node's receives: with a non-empty log it sends replicate (p0 = the
+                            log's length) to the lowest other block member.  replicate: lamport += p0, then
+                            replicate_ack (p0) to every other block member in index order; replicate_ack: nothing.
+                            Before init every message but init is received with no effect; a second init answers
+                            init_ok.  A message with in_reply_to is ignored; any other type gets error 10.  Replies
+                            carry in_reply_to only when the request had a msg_id.  One GPU. */
 enum { MS_TOPO_GRID = 0, MS_TOPO_LINE = 1, MS_TOPO_TOTAL = 2,                /* --topology, broadcast.clj:169-178 */
        MS_TOPO_TREE2 = 3, MS_TOPO_TREE3 = 4, MS_TOPO_TREE4 = 5 };
 enum { MS_DIST_CONSTANT = 0, MS_DIST_UNIFORM = 1, MS_DIST_EXPONENTIAL = 2 }; /* --latency-dist, net.clj:73-77 */
@@ -196,7 +216,8 @@ typedef struct ms_config {
   uint32_t seed_lo, seed_hi; /* Philox key; the reference is unseeded */
   double   p_loss;           /* net.clj:100 starts at 0; no CLI flag upstream */
   uint32_t n_values;         /* size of the value universe (seen-set bitmap bits per node) */
-  uint32_t gset_interval_ms; /* CRDT replication period: g-set (demo/ruby/g_set.rb:34), g-counter / pn-counter (crdt.rb) */
+  uint32_t gset_interval_ms; /* CRDT replication period: g-set (demo/ruby/g_set.rb:34), g-counter / pn-counter (crdt.rb);
+                              * the txn-rw-register node's replication period (0 = 100, txn_rw_register_hat.clj:110) */
   /* engine sizing (0 = default) */
   uint32_t max_endpoints;    /* servers + clients + services */
   uint32_t ring_cap;         /* per-endpoint inbox ring capacity, power of two */
@@ -213,7 +234,7 @@ typedef struct ms_config {
                               * in the size classes of windows up to 2048 */
   uint32_t n_shards;         /* GPUs the endpoints are sharded over (0/1 = single GPU), <= 8 */
   uint32_t shard_id;         /* this process's shard */
-  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn / proxy node (0 = 4096).  MS_W_KV_PROXY: [3] = the backing service MS_SVC_*, [4] = g for ms_add_kv_clients.  MS_W_KAFKA: [2] = keys per node (0 = 16, <= 65535), [3] = log capacity per key (0 = 4096), [4] = g for ms_add_kafka_clients (0 = 1).  MS_W_G_COUNTER / MS_W_PN_COUNTER: [4] = g, servers per block (0 = all, <= 1024) */
+  uint32_t reserved[6];      /* [0] = rounds of id history to keep (0 = default); [1] = 1: replay round batches from a CUDA graph; [2] = keys per service store / Raft KV (0 = 4096); [3] = Raft log capacity per node (0 = 4096); [4] = servers per Raft cluster: node_ids of a node's init = its block of g consecutive servers (0 = all servers, one cluster); [5] = pending-RPC table slots per Raft / txn / proxy node (0 = 4096).  MS_W_KV_PROXY: [3] = the backing service MS_SVC_*, [4] = g for ms_add_kv_clients.  MS_W_KAFKA: [2] = keys per node (0 = 16, <= 65535), [3] = log capacity per key (0 = 4096), [4] = g for ms_add_kafka_clients (0 = 1).  MS_W_G_COUNTER / MS_W_PN_COUNTER: [4] = g, servers per block (0 = all, <= 1024).  MS_W_TXN_RW: [2] = keys per node (0 = 1024, <= 16384), [3] = log capacity per node (0 = 4096), [4] = g, servers per block (0 = all, 2 <= g <= 32) */
   /* ABI 2.  Servers and the other endpoints (clients, hosts, services) may be sized apart: a
    * service hears from every node, a node from a few.  0 = ring_cap / max_window. */
   uint32_t server_ring_cap;  /* inbox ring capacity of the servers, power of two */
@@ -405,6 +426,64 @@ int64_t ms_kafka_committed(ms_sim* sim, uint32_t node, uint32_t key);
  * Copies at most cap entries into out and returns the count 2 x (the block's size); MS_ERR_ARG on another workload or a
  * bad node */
 int ms_counter_state(ms_sim* sim, uint32_t node, int64_t* out, size_t cap);
+
+/* Closed-loop txn-rw-register clients on the device (MS_W_TXN_RW, DESIGN.md 2.17): the client of
+ * workload/txn_rw_register.clj:108-136 with the generator below (Elle's is not in the reference).  The client side is
+ * that of ms_add_kafka_clients: one outstanding request, msg_id from 1, only in_reply_to is matched, timeout_ns.
+ *   binding  n_clients is a multiple of n_nodes; client k talks to server k mod n_nodes
+ *   draws    Philox(op, endpoint, 0xC11E47, 0): word 0 gives the length on [min_len, max_len], word 1 the stagger,
+ *            uniform on [0, 2 interval), bit i of word 3 makes micro-op i a write
+ *   keys     Philox(op, endpoint, 0xC11E47, 1): micro-op i takes key ((now / key_period_ns) * key_count +
+ *            ((word i * key_count) >> 32)) mod K, K = ms_config.reserved[2]: a function of virtual time
+ *   values   the client's j-th txn has base = 1 + 4 (k + n_clients j): micro-op i writes base + i, unique per key
+ *            (a base beyond 32 bits latches E_VALUE_RANGE)
+ *   outcome  with-errors #{}: a time-out or error code 0 / 13 is :info, any other code :fail; the client is reused
+ *   end      nothing is invoked at or after time_limit_ns; there is no final generator
+ *   history  ms_txn_rw_hist records in ms_txn_rw_history_drain */
+typedef struct ms_txn_rw_gen_config {
+  uint32_t n_clients;        /* a multiple of n_nodes */
+  uint32_t min_len, max_len; /* micro-ops per txn, 1 <= min_len <= max_len <= 4 */
+  uint32_t key_count;        /* keys in play at a time, 1 <= key_count <= reserved[2] */
+  int64_t  interval_ns;      /* mean delay between two ops of one client */
+  int64_t  timeout_ns;       /* 0 = 5 000 ms (client.clj:18-20) */
+  int64_t  time_limit_ns;    /* --time-limit */
+  int64_t  key_period_ns;    /* > 0: virtual time the clients spend on one set of keys */
+} ms_txn_rw_gen_config;
+typedef struct ms_txn_rw_hist {
+  int64_t  time_ns;
+  uint64_t order;            /* round << 24 | client ordinal, as ms_hist */
+  uint32_t client;           /* endpoint index */
+  uint32_t op;               /* the client's op counter: an invocation and its completion share it */
+  uint8_t  type;             /* MS_H_INVOKE / OK / FAIL / INFO */
+  uint8_t  f;                /* MS_HF_TXN_RW */
+  uint16_t error;            /* completion by an error reply: its code; MS_H_TIMEOUT for :net-timeout */
+  uint32_t node;             /* the server the client talks to */
+  uint32_t index;            /* ok: the txn's index in the node's log; else 0xFFFFFFFF */
+  uint32_t base;             /* micro-op i, a write, writes base + i */
+  uint64_t ops;              /* the micro-ops as in MS_T_TXN's p1 */
+  uint32_t reads[4];         /* ok: micro-op i, a read, returned reads[i] (0 = nil); else 0 */
+} ms_txn_rw_hist;
+enum { MS_HF_TXN_RW = 15 };
+/* adds cfg->n_clients endpoints "c<first_name> ..." and returns the index of the first.  MS_W_TXN_RW on one GPU, once
+ * per simulation, not together with the other closed-loop clients */
+int ms_add_txn_rw_clients(ms_sim* sim, const ms_txn_rw_gen_config* cfg, uint32_t first_name);
+/* The txn-rw-register clients' records in (time, round, client) order, as ms_history_drain */
+int ms_txn_rw_history_drain(ms_sim* sim, ms_txn_rw_hist* out, size_t cap, size_t* n_out);
+/* MS_W_TXN_RW: node's completed txns in log order.  Copies at most cap entries into out and returns the log's length;
+ * MS_ERR_ARG on another workload or a bad node */
+typedef struct ms_txn_rw_entry {
+  uint64_t lamport;          /* the txn's timestamp is [lamport, node] */
+  uint64_t ops;              /* the micro-ops as in MS_T_TXN's p1 */
+  uint32_t base;
+  uint32_t reads[4];         /* micro-op i, a read, returned reads[i] (0 = nil) */
+  uint32_t pad;
+} ms_txn_rw_entry;
+int ms_txn_rw_log(ms_sim* sim, uint32_t node, ms_txn_rw_entry* out, size_t cap);
+/* MS_W_TXN_RW: node's lamport clock, *log_len = its log's length, and its kv: value[k] (0 = nil) and ts[k], the
+ * lamport of the key's last write (the timestamp is [ts[k], node]; 0 where never written), for k < cap.  Returns K
+ * (ms_config.reserved[2]); MS_ERR_ARG as ms_txn_rw_log */
+int ms_txn_rw_state(ms_sim* sim, uint32_t node, uint64_t* lamport, uint32_t* log_len, uint32_t* value, uint64_t* ts,
+                    size_t cap);
 
 /* Upload a time-sorted schedule of client ops (appends). */
 int ms_schedule_ops(ms_sim* sim, const ms_op* ops, size_t n);

@@ -29,6 +29,8 @@ public final class Native {
   public static native long historyDrain(long h, ByteBuffer msHist32, long cap);
   public static native int addKafkaClients(long h, ByteBuffer msKafkaGenConfig, int firstName);
   public static native long kafkaHistoryDrain(long h, ByteBuffer msKafkaHist64, long cap);
+  public static native int addTxnRwClients(long h, ByteBuffer msTxnRwGenConfig, int firstName);
+  public static native long txnRwHistoryDrain(long h, ByteBuffer msTxnRwHist64, long cap);
   public static native int scheduleOps(long h, ByteBuffer msOps, long n);
   public static native int step(long h, long nRounds);
   public static native int run(long h, long untilNs);
@@ -63,6 +65,9 @@ public final class Native {
   public static native long kafkaLog(long h, int node, int key, ByteBuffer msgsU32, long cap);
   public static native long kafkaCommitted(long h, int node, int key);
   public static native int counterState(long h, int node, ByteBuffer outI64, long cap);
+  public static native int txnRwLog(long h, int node, ByteBuffer msTxnRwEntry40, long cap);
+  public static native int txnRwState(long h, int node, ByteBuffer lamportU64, ByteBuffer logLenU32, ByteBuffer valuesU32,
+                                      ByteBuffer tsU64, long cap);
   public static native int counters(long h, ByteBuffer out8);
   public static native int ringCounters(long h, ByteBuffer out, int n);
   public static native int setOrigin(long h, long round, long msgId, long eventId, int ringPos, int ringStride);

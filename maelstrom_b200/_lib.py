@@ -60,6 +60,12 @@ class KafkaGenConfig(C.Structure):   # ms_kafka_gen_config
                 ("pad", C.c_uint32), ("interval_ns", C.c_int64), ("timeout_ns", C.c_int64), ("time_limit_ns", C.c_int64)]
 
 
+class TxnRwGenConfig(C.Structure):   # ms_txn_rw_gen_config
+    _fields_ = [("n_clients", C.c_uint32), ("min_len", C.c_uint32), ("max_len", C.c_uint32), ("key_count", C.c_uint32),
+                ("interval_ns", C.c_int64), ("timeout_ns", C.c_int64), ("time_limit_ns", C.c_int64),
+                ("key_period_ns", C.c_int64)]
+
+
 class NemesisConfig(C.Structure):   # ms_nemesis_config
     _fields_ = [("group", C.c_uint32), ("targets", C.c_uint32), ("interval_ns", C.c_int64), ("start_ns", C.c_int64),
                 ("time_limit_ns", C.c_int64)]
@@ -72,6 +78,12 @@ KAFKA_HIST_DTYPE = np.dtype([("time_ns", "<i8"), ("order", "<u8"), ("client", "<
                              ("f", "u1"), ("error", "<u2"), ("key", "<u4", (2,)), ("a", "<u4", (2,)), ("b", "<u4", (2,)),
                              ("pad", "<u4", (3,))])
 assert KAFKA_HIST_DTYPE.itemsize == 64
+TXN_RW_HIST_DTYPE = np.dtype([("time_ns", "<i8"), ("order", "<u8"), ("client", "<u4"), ("op", "<u4"), ("type", "u1"),
+                              ("f", "u1"), ("error", "<u2"), ("node", "<u4"), ("index", "<u4"), ("base", "<u4"),
+                              ("ops", "<u8"), ("reads", "<u4", (4,))])
+assert TXN_RW_HIST_DTYPE.itemsize == 64
+TXN_RW_ENTRY_DTYPE = np.dtype([("lamport", "<u8"), ("ops", "<u8"), ("base", "<u4"), ("reads", "<u4", (4,)), ("pad", "<u4")])
+assert TXN_RW_ENTRY_DTYPE.itemsize == 40
 
 
 class JBatch(C.Structure):      # ms_jbatch
@@ -109,6 +121,10 @@ SYMBOLS = {
     "ms_kafka_log": (C.c_int, [_P, C.c_uint32, C.c_uint32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "ms_kafka_committed": (C.c_int64, [_P, C.c_uint32, C.c_uint32]),
     "ms_counter_state": (C.c_int, [_P, C.c_uint32, _P, C.c_size_t]),
+    "ms_add_txn_rw_clients": (C.c_int, [_P, _P, C.c_uint32]),
+    "ms_txn_rw_history_drain": (C.c_int, [_P, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "ms_txn_rw_log": (C.c_int, [_P, C.c_uint32, _P, C.c_size_t]),
+    "ms_txn_rw_state": (C.c_int, [_P, C.c_uint32, _P, _P, _P, _P, C.c_size_t]),
     "ms_schedule_ops": (C.c_int, [_P, _P, C.c_size_t]),
     "ms_step": (C.c_int, [_P, C.c_uint64]),
     "ms_run": (C.c_int, [_P, C.c_int64]),

@@ -22,7 +22,7 @@ enum : uint32_t {
   E_NONE = 0, E_RING_OVERFLOW = 1, E_WINDOW_OVERFLOW = 2, E_JOURNAL_OVERFLOW = 3,
   E_INVALID_DEST = 4, E_HISTORY = 5, E_VALUE_RANGE = 6, E_MAIL_OVERFLOW = 7,
   E_CALENDAR_OVERFLOW = 8, E_ID_RANGE = 9, E_BARRIER = 10, E_SNAPSHOT = 11,
-  E_RAFT_CAPACITY = 12, E_HISTORY_RING = 13, E_KAFKA_CAPACITY = 14
+  E_RAFT_CAPACITY = 12, E_HISTORY_RING = 13, E_KAFKA_CAPACITY = 14, E_TXN_RW_CAPACITY = 15
 };
 
 // Mutable per-simulation scalars, resident in HBM, committed by the last CTA of
@@ -275,6 +275,18 @@ struct Params {
   int64_t*  ct_val;          // [n_servers][2 * ct_width]
   int64_t*  ct_snap;         // [n_servers * gs_slots][2 * ct_width]
   uint32_t  ct_width, ct_pad;
+  // MS_W_TXN_RW (rw_handle in csrc/ms_raft.cuh): per node its lamport clock, its kv (value, then the lamport of the
+  // write) and the log of its completed txns, whose length also stands for the unreplicated map; the replication task
+  // fires at gs_next_fire (g-set's array).  Block size in rf_group; the clients share gc and kafka's 64-B history ring
+  // (kf_hist).  Appended
+  uint64_t* rw_lamport;      // [n_servers]
+  uint32_t* rw_val;          // [n_servers][rw_keys]
+  uint64_t* rw_ts;           // [n_servers][rw_keys]
+  ms_txn_rw_entry* rw_log;   // [n_servers][rw_cap]
+  uint32_t* rw_len;          // [n_servers]
+  uint32_t  rw_keys, rw_cap;
+  uint32_t  rw_min_len, rw_max_len, rw_key_count, rw_pad;
+  int64_t   rw_key_period_ns;
 };
 
 constexpr uint32_t kRaftCallbacks = 4096;       // default pending-RPC table slots per node (ms_config.reserved[5]; oracle: same)
@@ -320,11 +332,13 @@ struct GenDev {
   uint32_t node;                       // the server this client talks to
   uint32_t ops;                        // ops invoked so far
   union { uint32_t bcasts;             // broadcasts among them
-          uint32_t key_base; };        // lin-kv client: first key of its group's range
+          uint32_t key_base;           // lin-kv client: first key of its group's range
+          uint32_t ops_lo; };          // txn-rw-register client: the micro-ops of the txn in flight, low half
   uint32_t phase;                      // 0 mix, 1 quiet period, 2 final read outstanding, 3 done
   uint32_t cur_f, cur_value;           // the op in flight
   uint32_t ordinal;                    // k of client k
-  uint32_t reader;                     // lin-kv client: 1 = only reads (gen/reserve)
+  union { uint32_t reader;             // lin-kv client: 1 = only reads (gen/reserve)
+          uint32_t ops_hi; };          // txn-rw-register client: the micro-ops, high half
 };
 enum : uint32_t { GEN_MIX = 0, GEN_QUIET = 1, GEN_FINAL = 2, GEN_DONE = 3 };
 

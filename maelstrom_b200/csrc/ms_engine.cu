@@ -95,6 +95,7 @@ static const char* dev_error_text(uint32_t code) {
     case E_BARRIER: return "cross-shard barrier timed out waiting for shard";
     case E_RAFT_CAPACITY: return "Raft node out of log / staging / payload-heap capacity (raise ms_config.reserved[3]) at node";
     case E_KAFKA_CAPACITY: return "kafka node's log of a key is full (raise ms_config.reserved[3]) at node";
+    case E_TXN_RW_CAPACITY: return "txn-rw-register node's log is full (raise ms_config.reserved[3]) at node";
     case E_HISTORY_RING: return "history ring of the closed-loop clients is full (call ms_history_drain more often) at client";
     case E_SNAPSHOT: return "replicate_full names a set snapshot that is not resident (in flight longer than calendar_slots, or forged), or a merge a counter snapshot that is not: sender";
   }
@@ -610,7 +611,7 @@ static int build_sim(ms_sim* s, const ms_config* in) {
   ms_config& c = s->cfg;
   c = *in;
   if (c.n_nodes == 0) { set_err("n_nodes must be positive (--node-count)"); return MS_ERR_ARG; }
-  if (c.workload > MS_W_PN_COUNTER || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
+  if (c.workload > MS_W_TXN_RW || c.topology > MS_TOPO_TREE4 || c.latency_dist > MS_DIST_EXPONENTIAL) {
     set_err("bad workload/topology/latency_dist");
     return MS_ERR_ARG;
   }
@@ -638,7 +639,7 @@ static int build_sim(ms_sim* s, const ms_config* in) {
   if (c.journal_level > 2) c.journal_level = 2;
   if (!c.mailbox_cap) c.mailbox_cap = 1u << 16;
   if (!c.inject_cap) c.inject_cap = 1u << 16;
-  if (!c.gset_interval_ms) c.gset_interval_ms = 5000;
+  if (!c.gset_interval_ms) c.gset_interval_ms = c.workload == MS_W_TXN_RW ? 100u : 5000u;   // (Thread/sleep 100), g_set.rb:34
   s->use_calendar = c.latency_mean_ms > 0;
   if (s->use_calendar) {
     c.calendar_slots = pow2_at_least(c.calendar_slots ? c.calendar_slots
@@ -846,6 +847,33 @@ static int build_sim(ms_sim* s, const ms_config* in) {
         (rc = s->dalloc(&P.gs_init, N)) || (rc = s->dalloc(&P.gs_next_fire, N)) || (rc = s->dalloc(&P.gs_fires, N)) ||
         (rc = s->dalloc(&P.gs_tag, rows)) || (rc = s->dalloc(&P.ct_val, N * 2 * g)) || (rc = s->dalloc(&P.ct_snap, rows * 2 * g)))
       return rc;
+  }
+  if (c.workload == MS_W_TXN_RW) {
+    // txn-rw-register nodes (rw_handle, csrc/ms_raft.cuh): per node its lamport clock, kv and log; the replication
+    // task's schedule; the staging rows of the sequential step.  A message brings at most max(1, g - 1) sends (a
+    // reply, or the acks of a replicate), the task one more: the rows hold the bound, and rf_emit latches beyond it
+    if (c.n_shards > 1) { set_err("MS_W_TXN_RW runs on one GPU"); return MS_ERR_ARG; }
+    const uint32_t g = c.reserved[4] ? c.reserved[4] : c.n_nodes;
+    if (g < 2 || g > 32 || c.n_nodes % g) {
+      set_err("MS_W_TXN_RW: blocks of 2 to 32 servers that divide n_nodes (ms_config.reserved[4], 0 = all servers)");
+      return MS_ERR_ARG;
+    }
+    P.rw_keys = c.reserved[2] ? c.reserved[2] : 1024u;
+    P.rw_cap = c.reserved[3] ? c.reserved[3] : 4096u;
+    if (P.rw_keys > 16384u) { set_err("MS_W_TXN_RW: ms_config.reserved[2] (keys per node) must be <= 16384"); return MS_ERR_ARG; }
+    const size_t N = c.n_nodes;
+    P.rf_group = g < c.n_nodes ? g : 0u;
+    P.rf_stage_cap = c.server_max_window * std::max(1u, g - 1u) + 1u;
+    P.rf_cb_mask = 0;
+    P.gs_interval_ms = c.gset_interval_ms;
+    if ((rc = s->dalloc(&P.rf_node, N)) || (rc = s->dalloc(&P.rf_cb, N * 2)) || (rc = s->dalloc(&P.rf_stage, N * P.rf_stage_cap * 3)) ||
+        (rc = s->dalloc(&P.gs_next_fire, N)) || (rc = s->dalloc(&P.rw_lamport, N)) || (rc = s->dalloc(&P.rw_val, N * P.rw_keys)) ||
+        (rc = s->dalloc(&P.rw_ts, N * P.rw_keys)) || (rc = s->dalloc(&P.rw_log, N * P.rw_cap)) || (rc = s->dalloc(&P.rw_len, N)))
+      return rc;
+    // the replication thread starts with the node's process, at virtual time 0: first run at one period
+    std::vector<int64_t> fire(N, (int64_t)c.gset_interval_ms * kTickNs);
+    CK(cudaMemcpyAsync(P.gs_next_fire, fire.data(), N * 8, cudaMemcpyHostToDevice, s->stream));
+    CK(cudaStreamSynchronize(s->stream));
   }
   if (c.workload == MS_W_TXN || c.workload == MS_W_TXN_TREE || c.workload == MS_W_KV_PROXY) {
     // txn-list-append nodes and lin-kv proxies: message ids, the table of pending RPC closures and the staging rows
@@ -1305,7 +1333,16 @@ int ms_add_kafka_clients(ms_sim* s, const ms_kafka_gen_config* kc, uint32_t firs
   return (int)first;
 }
 
-int ms_kafka_history_drain(ms_sim* s, ms_kafka_hist* out, size_t cap, size_t* n_out) {
+// The ring of 64-B history records of the kafka and the txn-rw-register clients (one kind per simulation): every
+// record starts with time_ns and order
+struct Hist64 {
+  int64_t  time_ns;
+  uint64_t order;
+  uint32_t rest[12];
+};
+static_assert(sizeof(Hist64) == 64 && sizeof(ms_kafka_hist) == 64 && sizeof(ms_txn_rw_hist) == 64,
+              "a 64-B history record is the device record");
+static int hist64_drain(ms_sim* s, Hist64* out, size_t cap, size_t* n_out) {
   std::lock_guard<std::mutex> g(s->mu);
   cudaSetDevice(s->device);
   if (n_out) *n_out = 0;
@@ -1313,7 +1350,6 @@ int ms_kafka_history_drain(ms_sim* s, ms_kafka_hist* out, size_t cap, size_t* n_
   const uint64_t avail = s->hs.kf_hist_n - s->hs.kf_hist_drained;
   const size_t n = (size_t)std::min<uint64_t>(avail, cap);
   if (!n || !out) return MS_OK;
-  static_assert(sizeof(ms_kafka_hist) == 64, "ms_kafka_hist is the device record");
   for (size_t k = 0; k < n;) {      // the ring may wrap
     const uint64_t pos = (s->hs.kf_hist_drained + k) & s->P.kf_hist_mask;
     const size_t piece = (size_t)std::min<uint64_t>(n - k, (uint64_t)s->P.kf_hist_mask + 1 - pos);
@@ -1321,13 +1357,17 @@ int ms_kafka_history_drain(ms_sim* s, ms_kafka_hist* out, size_t cap, size_t* n_
     k += piece;
   }
   // as ms_history_drain: (time, round, client) is the order; one client's records of a round keep theirs
-  std::stable_sort(out, out + n, [](const ms_kafka_hist& a, const ms_kafka_hist& b) {
+  std::stable_sort(out, out + n, [](const Hist64& a, const Hist64& b) {
     return a.time_ns != b.time_ns ? a.time_ns < b.time_ns : a.order < b.order;
   });
   s->hs.kf_hist_drained += n;
   CK(cudaMemcpy(&s->P.st->kf_hist_drained, &s->hs.kf_hist_drained, 8, cudaMemcpyHostToDevice));
   if (n_out) *n_out = n;
   return MS_OK;
+}
+
+int ms_kafka_history_drain(ms_sim* s, ms_kafka_hist* out, size_t cap, size_t* n_out) {
+  return hist64_drain(s, reinterpret_cast<Hist64*>(out), cap, n_out);
 }
 
 static int kafka_slot(ms_sim* s, uint32_t node, uint32_t key, const char* what) {
@@ -1363,6 +1403,99 @@ int64_t ms_kafka_committed(ms_sim* s, uint32_t node, uint32_t key) {
   CK(cudaStreamSynchronize(s->stream));
   CK(cudaMemcpy(&c, s->P.kf_committed + (size_t)node * s->P.kf_keys + key, 4, cudaMemcpyDeviceToHost));
   return c == kKafkaAbsent ? -1 : (int64_t)c;
+}
+
+// Closed-loop txn-rw-register clients: n endpoints "c<first_name>..", client k on server k mod n, driven by rw_gen_step
+// inside the sequential family's round kernel (csrc/ms_kernels.cu); their records share the kafka clients' ring.
+int ms_add_txn_rw_clients(ms_sim* s, const ms_txn_rw_gen_config* rc_, uint32_t first_name) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  if (s->cfg.workload != MS_W_TXN_RW) { set_err("ms_add_txn_rw_clients: the txn-rw-register clients drive the MS_W_TXN_RW nodes"); return MS_ERR_ARG; }
+  Params& P = s->P;
+  if (!rc_ || rc_->n_clients == 0 || rc_->interval_ns <= 0 || rc_->timeout_ns < 0 || rc_->key_period_ns <= 0 ||
+      rc_->min_len < 1 || rc_->min_len > rc_->max_len || rc_->max_len > 4 || rc_->key_count == 0 || rc_->key_count > P.rw_keys) {
+    set_err("ms_add_txn_rw_clients: bad configuration (1 <= min_len <= max_len <= 4, 1 <= key_count <= ms_config.reserved[2], "
+            "interval_ns and key_period_ns > 0)");
+    return MS_ERR_ARG;
+  }
+  if (P.gc) { set_err("ms_add_txn_rw_clients: the generator's clients exist already"); return MS_ERR_ARG; }
+  if (rc_->n_clients % s->cfg.n_nodes) {
+    set_err("ms_add_txn_rw_clients: n_clients must be a multiple of n_nodes (" + std::to_string(s->cfg.n_nodes) + ")");
+    return MS_ERR_ARG;
+  }
+  if ((uint64_t)P.n_ep + rc_->n_clients > s->cfg.max_endpoints) { set_err("max_endpoints exhausted"); return MS_ERR_CAPACITY; }
+  for (uint32_t k = 0; k < rc_->n_clients; k++)
+    if (s->by_name.count("c" + std::to_string(first_name + k))) { set_err("endpoint already exists: c" + std::to_string(first_name + k)); return MS_ERR_ARG; }
+  int rc;
+  // a client writes at most two records per round (a completion and the next invocation)
+  const uint32_t hist_cap = pow2_at_least(std::max<uint32_t>(1u << 16, 64u * rc_->n_clients));
+  if ((rc = s->dalloc(&P.gc, s->cfg.max_endpoints)) || (rc = s->dalloc(&P.kf_hist, (size_t)hist_cap * 4))) return rc;
+  P.kf_hist_mask = hist_cap - 1u;
+  P.gc_n = rc_->n_clients;
+  P.gc_interval_ns = rc_->interval_ns;
+  P.gc_timeout_ns = rc_->timeout_ns > 0 ? rc_->timeout_ns : 5000ll * kTickNs;   // client.clj:18-20
+  P.gc_limit_ns = rc_->time_limit_ns;
+  P.rw_min_len = rc_->min_len;
+  P.rw_max_len = rc_->max_len;
+  P.rw_key_count = rc_->key_count;
+  P.rw_key_period_ns = rc_->key_period_ns;
+  const uint32_t first = P.n_ep;
+  std::vector<GenDev> init(rc_->n_clients);
+  memset(init.data(), 0, init.size() * sizeof(GenDev));
+  for (uint32_t k = 0; k < rc_->n_clients; k++) {
+    const std::string id = "c" + std::to_string(first_name + k);
+    const uint32_t idx = first + k;
+    s->kinds[idx] = MS_KIND_GEN_CLIENT;
+    s->names.push_back(id);
+    s->mailbox.emplace_back();
+    s->by_name[id] = idx;
+    init[k].node = k % s->cfg.n_nodes;
+    init[k].ordinal = k;
+  }
+  P.n_ep = first + rc_->n_clients;
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(P.kind + first, s->kinds.data() + first, rc_->n_clients, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(P.gc + first, init.data(), init.size() * sizeof(GenDev), cudaMemcpyHostToDevice));
+  return (int)first;
+}
+
+int ms_txn_rw_history_drain(ms_sim* s, ms_txn_rw_hist* out, size_t cap, size_t* n_out) {
+  return hist64_drain(s, reinterpret_cast<Hist64*>(out), cap, n_out);
+}
+
+static int txn_rw_node(ms_sim* s, uint32_t node, const char* what) {
+  if (s->cfg.workload != MS_W_TXN_RW || node >= s->cfg.n_nodes) {
+    set_err(std::string(what) + ": not a txn-rw-register node (MS_W_TXN_RW, node < n_nodes)");
+    return MS_ERR_ARG;
+  }
+  return MS_OK;
+}
+
+int ms_txn_rw_log(ms_sim* s, uint32_t node, ms_txn_rw_entry* out, size_t cap) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  int rc;
+  if ((rc = txn_rw_node(s, node, "ms_txn_rw_log"))) return rc;
+  uint32_t n = 0;
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(&n, s->P.rw_len + node, 4, cudaMemcpyDeviceToHost));
+  const size_t m = std::min<size_t>(n, out ? cap : 0);
+  if (m) CK(cudaMemcpy(out, s->P.rw_log + (size_t)node * s->P.rw_cap, m * sizeof(ms_txn_rw_entry), cudaMemcpyDeviceToHost));
+  return (int)n;
+}
+
+int ms_txn_rw_state(ms_sim* s, uint32_t node, uint64_t* lamport, uint32_t* log_len, uint32_t* value, uint64_t* ts, size_t cap) {
+  std::lock_guard<std::mutex> g(s->mu);
+  cudaSetDevice(s->device);
+  int rc;
+  if ((rc = txn_rw_node(s, node, "ms_txn_rw_state"))) return rc;
+  const size_t K = s->P.rw_keys, m = std::min<size_t>(K, cap);
+  CK(cudaStreamSynchronize(s->stream));
+  if (lamport) CK(cudaMemcpy(lamport, s->P.rw_lamport + node, 8, cudaMemcpyDeviceToHost));
+  if (log_len) CK(cudaMemcpy(log_len, s->P.rw_len + node, 4, cudaMemcpyDeviceToHost));
+  if (value && m) CK(cudaMemcpy(value, s->P.rw_val + node * K, m * 4, cudaMemcpyDeviceToHost));
+  if (ts && m) CK(cudaMemcpy(ts, s->P.rw_ts + node * K, m * 8, cudaMemcpyDeviceToHost));
+  return (int)K;
 }
 
 int ms_counter_state(ms_sim* s, uint32_t node, int64_t* out, size_t cap) {
@@ -1842,8 +1975,9 @@ int ms_set_nemesis(ms_sim* s, const ms_nemesis_config* nc) {
   if (s->cfg.reserved[1] == 1) { set_err("ms_set_nemesis: not with CUDA-graph replay (ms_config.reserved[1] = 1)"); return MS_ERR_ARG; }
   if (s->np.comp_active) { set_err("ms_set_nemesis: a bulk partition is installed (ms_net_heal first)"); return MS_ERR_ARG; }
   const uint32_t N = s->cfg.n_nodes;
-  // Raft clusters and counter blocks are closed under the nodes' traffic
-  const bool blocks = s->cfg.workload == MS_W_RAFT || s->cfg.workload == MS_W_G_COUNTER || s->cfg.workload == MS_W_PN_COUNTER;
+  // Raft clusters, counter and txn-rw-register blocks are closed under the nodes' traffic
+  const bool blocks = s->cfg.workload == MS_W_RAFT || s->cfg.workload == MS_W_G_COUNTER || s->cfg.workload == MS_W_PN_COUNTER ||
+                      s->cfg.workload == MS_W_TXN_RW;
   const uint32_t natural = (blocks && P.rf_group) ? P.rf_group : N;
   const uint32_t gsz = nc->group ? nc->group : natural;
   if (gsz != natural || gsz == 0 || gsz > kNemMaxGroup) {

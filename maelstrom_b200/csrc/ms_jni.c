@@ -114,6 +114,16 @@ jlong FN(kafkaHistoryDrain)(JNIEnv* env, jclass c, jlong h, jobject out, jlong c
   const int rc = ms_kafka_history_drain(H(h), (ms_kafka_hist*)BUF(out), (size_t)cap, &n);
   return rc < 0 ? (jlong)rc : (jlong)n;
 }
+jint FN(addTxnRwClients)(JNIEnv* env, jclass c, jlong h, jobject cfg, jint firstName) {
+  (void)c;
+  return ms_add_txn_rw_clients(H(h), (const ms_txn_rw_gen_config*)BUF(cfg), (uint32_t)firstName);
+}
+jlong FN(txnRwHistoryDrain)(JNIEnv* env, jclass c, jlong h, jobject out, jlong cap) {
+  (void)c;
+  size_t n = 0;
+  const int rc = ms_txn_rw_history_drain(H(h), (ms_txn_rw_hist*)BUF(out), (size_t)cap, &n);
+  return rc < 0 ? (jlong)rc : (jlong)n;
+}
 jint FN(scheduleOps)(JNIEnv* env, jclass c, jlong h, jobject ops, jlong n) {
   (void)c;
   return ms_schedule_ops(H(h), (const ms_op*)BUF(ops), (size_t)n);
@@ -228,6 +238,19 @@ jlong FN(kafkaCommitted)(JNIEnv* env, jclass c, jlong h, jint node, jint key) { 
 jint FN(counterState)(JNIEnv* env, jclass c, jlong h, jint node, jobject out, jlong cap) {
   (void)c;
   return ms_counter_state(H(h), (uint32_t)node, out ? (int64_t*)BUF(out) : NULL, (size_t)cap);
+}
+/* txn-rw-register read-backs: out = direct buffer of cap 40-B ms_txn_rw_entry; returns the log's length or a negative
+ * error */
+jint FN(txnRwLog)(JNIEnv* env, jclass c, jlong h, jint node, jobject out, jlong cap) {
+  (void)c;
+  return ms_txn_rw_log(H(h), (uint32_t)node, out ? (ms_txn_rw_entry*)BUF(out) : NULL, (size_t)cap);
+}
+/* lamport = direct buffer of one u64, logLen of one u32, values of cap u32, ts of cap u64; returns K or a negative error */
+jint FN(txnRwState)(JNIEnv* env, jclass c, jlong h, jint node, jobject lamport, jobject logLen, jobject values, jobject ts,
+                    jlong cap) {
+  (void)c;
+  return ms_txn_rw_state(H(h), (uint32_t)node, (uint64_t*)BUF(lamport), (uint32_t*)BUF(logLen), (uint32_t*)BUF(values),
+                         (uint64_t*)BUF(ts), (size_t)cap);
 }
 jint FN(counters)(JNIEnv* env, jclass c, jlong h, jobject out8) { (void)c; return ms_counters(H(h), (uint64_t*)BUF(out8)); }
 /* out = direct buffer of n u64 (>= 6 x n_nodes): tail / limit / head of the 48-B rings, then of the compact rings */

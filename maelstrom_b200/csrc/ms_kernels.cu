@@ -824,6 +824,86 @@ __device__ bool ct_gen_step(const Params& p, DevState* st, uint32_t e, int64_t n
   return send;
 }
 
+// The txn-rw-register client (ms_add_txn_rw_clients, DESIGN.md 2.17): the client side of kv_gen_step with the client
+// of workload/txn_rw_register.clj:108-136 and the generator of the header; the oracle's twin is
+// tests/native/txn_rw_oracle.cpp.  cur_value holds the txn's base, ops_lo / ops_hi its micro-ops; the records go to
+// kafka's ring of 64-B records.  GenDev keeps kv_gen_step's meaning: gen_timer_due and gen_wake_ns hold for it as they are.
+__device__ void rw_hist(const Params& p, DevState* st, int64_t now, uint64_t round, uint32_t e, const GenDev& g,
+                        uint32_t type, uint32_t error, uint32_t index, const uint32_t reads[4]) {
+  const unsigned long long pos = atomicAdd((unsigned long long*)&st->kf_hist_n, 1ull);
+  if (pos - st->kf_hist_drained > p.kf_hist_mask) { latch_error(st, E_HISTORY_RING, e); return; }
+  uint4* at = p.kf_hist + (pos & p.kf_hist_mask) * 4;
+  const uint64_t order = (round << 24) | g.ordinal;
+  at[0] = make_uint4((uint32_t)now, (uint32_t)((uint64_t)now >> 32), (uint32_t)order, (uint32_t)(order >> 32));
+  at[1] = make_uint4(e, g.ops, type | ((uint32_t)MS_HF_TXN_RW << 8) | (error << 16), g.node);
+  at[2] = make_uint4(index, g.cur_value, g.ops_lo, g.ops_hi);
+  at[3] = make_uint4(reads[0], reads[1], reads[2], reads[3]);
+}
+
+__device__ bool rw_gen_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const uint4* myring,
+                            uint32_t head, uint32_t my_mask, uint32_t n, const uint16_t* ord, const uint32_t* vals, Rec& out) {
+  GenDev g = p.gc[e];
+  const uint32_t none[4] = {0u, 0u, 0u, 0u};
+  for (uint32_t pos = 0; pos < n; pos++) {
+    const uint32_t i = ord[pos];
+    if (!(vals[i] & (1u << 30))) continue;                                 // V_RECV: cut by a partition
+    const uint4* rp = myring + (size_t)((head + i) & my_mask) * 3;
+    const uint4 vb = rp[1], vc = rp[2];
+    const uint32_t type = vc.x & 0xFFFFu, flags = vc.x >> 16;
+    if (!g.waiting_for || !(flags & MS_F_REPLY) || vb.w != g.waiting_for) continue;   // client.clj:106-107
+    g.waiting_for = 0;
+    if (type == MS_T_ERROR) {                                              // with-errors #{} (:116)
+      const uint32_t err = vc.y;
+      rw_hist(p, st, now, round, e, g, err == 0 || err == 13 ? MS_H_INFO : MS_H_FAIL, err, 0xFFFFFFFFu, none);
+      continue;
+    }
+    const uint32_t index = vc.y;                                           // txn_ok: the entry of the node's log
+    if (index >= p.rw_cap) { latch_error(st, E_VALUE_RANGE, index); continue; }
+    const ms_txn_rw_entry en = p.rw_log[(size_t)g.node * p.rw_cap + index];
+    rw_hist(p, st, now, round, e, g, MS_H_OK, 0, index, en.reads);
+  }
+  if (g.waiting_for && now >= g.deadline_ns) {                             // :net-timeout
+    rw_hist(p, st, now, round, e, g, MS_H_INFO, MS_H_TIMEOUT, 0xFFFFFFFFu, none);
+    g.waiting_for = 0;
+  }
+  bool send = false;
+  if (!g.waiting_for && g.phase == GEN_MIX) {
+    if (now >= p.gc_limit_ns) {
+      g.phase = GEN_DONE;
+    } else if (now >= g.next_op_ns) {
+      uint32_t x[4], y[4];
+      philox4x32_10(g.ops, e, 0xC11E47u, 0u, p.seed_lo, p.seed_hi, x);     // the client's own stream: op k
+      philox4x32_10(g.ops, e, 0xC11E47u, 1u, p.seed_lo, p.seed_hi, y);     // and its keys
+      const uint64_t base = 1ull + 4ull * (g.ordinal + (uint64_t)p.gc_n * g.ops);
+      if (base + 3ull > 0xFFFFFFFFull) {
+        latch_error(st, E_VALUE_RANGE, e);
+      } else {
+        const uint32_t len = p.rw_min_len + (uint32_t)(((uint64_t)x[0] * (p.rw_max_len - p.rw_min_len + 1u)) >> 32);
+        const uint64_t slot = (uint64_t)(now / p.rw_key_period_ns) % p.rw_keys * p.rw_key_count;
+        uint64_t ops = 0;
+        for (uint32_t m = 0; m < len; m++) {
+          const uint32_t key = (uint32_t)((slot + (((uint64_t)y[m] * p.rw_key_count) >> 32)) % p.rw_keys);
+          ops |= (uint64_t)(0x8000u | ((x[3] >> m) & 1u) << 14 | key) << (16 * m);
+        }
+        g.next_op_ns = now + (int64_t)(((unsigned __int128)x[1] * (unsigned __int128)(2 * (uint64_t)p.gc_interval_ns)) >> 32);
+        g.ops++;
+        g.cur_f = MS_HF_TXN_RW; g.cur_value = (uint32_t)base;
+        g.ops_lo = (uint32_t)ops; g.ops_hi = (uint32_t)(ops >> 32);
+        g.waiting_for = ++g.next_msg_id;                                   // client.clj:61-64
+        g.deadline_ns = now + p.gc_timeout_ns;
+        rw_hist(p, st, now, round, e, g, MS_H_INVOKE, 0, 0xFFFFFFFFu, none);
+        out.round = 0; out.ticket = 0; out.idx = 0;
+        out.src = e; out.dest = g.node; out.msg_id = g.waiting_for; out.in_reply_to = 0;
+        out.tf = MS_T_TXN | ((uint32_t)MS_F_MSG_ID << 16);
+        out.p0 = (uint32_t)base; out.p1 = ops;
+        send = true;
+      }
+    }
+  }
+  p.gc[e] = g;
+  return send;
+}
+
 #include "ms_tree.h"
 #include "ms_raft.cuh"
 
@@ -937,11 +1017,14 @@ __device__ void snapshot_endpoints(const Params& p, DevState* st, uint32_t gid, 
       n += cl - ch;
     }
     if (p.kind[e] & kRemoved) n = 0;
-    // g-set, g-counter / pn-counter: a node whose periodic replication task is due emits even with an empty window
+    // g-set, g-counter / pn-counter, txn-rw-register: a node whose periodic replication task is due (and, for
+    // txn-rw-register, has something to replicate) emits even with an empty window
     // Raft: a node whose election / step-down / replication timers are due acts on an empty window too
     const bool timer_due = e < p.n_servers && p.kind[e] == MS_KIND_SERVER &&
                            ((p.workload == MS_W_GSET && p.gs_init[e] && st->now >= p.gs_next_fire[e]) ||
-                            (p.workload >= MS_W_G_COUNTER && p.gs_init[e] && st->now >= p.gs_next_fire[e]) ||
+                            ((p.workload == MS_W_G_COUNTER || p.workload == MS_W_PN_COUNTER) && p.gs_init[e] &&
+                             st->now >= p.gs_next_fire[e]) ||
+                            (p.workload == MS_W_TXN_RW && p.rw_len[e] && st->now >= p.gs_next_fire[e]) ||
                             (p.workload == MS_W_RAFT && rf_timer_due(p.rf_node[e], st->now)) ||
                             (p.workload == MS_W_TXN_TREE && tt_timer_due(p.tt_node[e], st->now)));
     const bool gen_due = p.gc && p.kind[e] == MS_KIND_GEN_CLIENT && gen_timer_due(p, p.gc[e], st->now);
@@ -1005,7 +1088,8 @@ __global__ void k_wake(Params p) {
     // snapshot_endpoints' timer_due / gen_due
     if (e < p.n_servers && p.kind[e] == MS_KIND_SERVER) {
       if (p.workload == MS_W_GSET && p.gs_init[e]) w = min(w, p.gs_next_fire[e]);
-      if (p.workload >= MS_W_G_COUNTER && p.gs_init[e]) w = min(w, p.gs_next_fire[e]);
+      if ((p.workload == MS_W_G_COUNTER || p.workload == MS_W_PN_COUNTER) && p.gs_init[e]) w = min(w, p.gs_next_fire[e]);
+      if (p.workload == MS_W_TXN_RW && p.rw_len[e]) w = min(w, p.gs_next_fire[e]);
       if (p.workload == MS_W_RAFT) w = min(w, rf_wake_ns(p.rf_node[e]));
       if (p.workload == MS_W_TXN_TREE) w = min(w, tt_wake_ns(p.tt_node[e]));
     }
@@ -1856,14 +1940,15 @@ __device__ void service_handle(const Params& p, uint32_t svc, const SvReq& q, ui
 }
 
 // ------------------------------------------------------------------ node programs run by k_round
-// Raft / txn-list-append / proxy / kafka / counter server e (ms_raft.cuh), one thread: the window in id order, then the node's timers.
+// Raft / txn-list-append / proxy / kafka / counter / txn-rw-register server e (ms_raft.cuh), one thread: the window in id order, then the node's timers.
 // Returns the number of sends it staged in rf_stage; k_round emits them.
 __device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t now, uint64_t round, const Win& w,
                               uint32_t n, const RoundSmem& sm) {
   RaftCtx c{p, st, e, now, round, p.rf_node + e, p.rf_log + (size_t)e * p.rf_log_cap * 2,
             p.rf_cb + (size_t)e * (p.rf_cb_mask + 1u) * 2, p.rf_stage + (size_t)e * p.rf_stage_cap * 3, 0u, 0u, 0u, 0u};
   rf_group_of(p, e, c.gbase, c.gn);
-  if (p.workload >= MS_W_G_COUNTER) ct_task(c);                  // the counter's replication task: before its receives
+  if (p.workload == MS_W_G_COUNTER || p.workload == MS_W_PN_COUNTER) ct_task(c);   // the replication tasks: before
+  if (p.workload == MS_W_TXN_RW) rw_task(c);                                          // the node's receives
   for (uint32_t pos = 0; pos < n; pos++) {
     const uint32_t i = sm.ord[pos];
     if (!(sm.vals[i] & V_RECV)) continue;
@@ -1872,7 +1957,8 @@ __device__ uint32_t raft_step(const Params& p, DevState* st, uint32_t e, int64_t
     else if (p.workload == MS_W_TXN_TREE) tt_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else if (p.workload == MS_W_KV_PROXY) kp_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else if (p.workload == MS_W_KAFKA) kf_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
-    else if (p.workload >= MS_W_G_COUNTER) ct_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+    else if (p.workload == MS_W_G_COUNTER || p.workload == MS_W_PN_COUNTER) ct_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
+    else if (p.workload == MS_W_TXN_RW) rw_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
     else txn_handle(c, rec_unpack(rp[0], rp[1], rp[2]));
   }
   if (p.workload == MS_W_RAFT) { rf_actions(c); rf_note_busy(c); }
@@ -2464,11 +2550,14 @@ __global__ void __launch_bounds__(CLS == 3 ? 512 : 256, CLS == 3 ? 2 : MS_ROUND_
       if (tid == 0) {
         Rec q;
         bool send;
-        // the Raft family's clients are the lin-kv ones (ms_add_kv_clients), the kafka ones (ms_add_kafka_clients) or
-        // the counter ones (ms_add_gen_clients); their requests carry a p1
+        // the Raft family's clients are the lin-kv ones (ms_add_kv_clients), the kafka ones (ms_add_kafka_clients),
+        // the counter ones (ms_add_gen_clients) or the txn-rw-register ones (ms_add_txn_rw_clients); their requests
+        // carry a p1
         if constexpr (RF) send = p.workload == MS_W_KAFKA ? kf_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q)
-                               : p.workload >= MS_W_G_COUNTER ? ct_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q)
-                                                              : kv_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
+                               : p.workload == MS_W_G_COUNTER || p.workload == MS_W_PN_COUNTER
+                                   ? ct_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q)
+                               : p.workload == MS_W_TXN_RW ? rw_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q)
+                                                           : kv_gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
         else send = gen_step(p, st, e, now, round, myring, head, my_mask, n, ord, vals, q);
         if (send) {
           s_gen[0] = make_uint4(q.src, q.dest, q.msg_id, q.in_reply_to);

@@ -687,6 +687,86 @@ __device__ void ct_handle(RaftCtx& c, const Rec& m) {
   rf_emit(c, a);
 }
 
+// ------------------------------------------------------------------ txn-rw-register
+// demo/clojure/txn_rw_register_hat.clj on node.clj (DESIGN.md 2.17).  node.clj:178 parses a message with string keys
+// and keywordizes only the top level and the body (:165-171), so a replicate's txn+s are string-keyed maps: apply-txn+!
+// finds neither :ts nor :txn (:40) and applies an empty txn under a fresh timestamp, nothing enters the receiver's
+// unreplicated map, and the acks carry nil timestamps that remove nothing (:145,157).  A node's unreplicated map is
+// therefore every txn it has served, each pending at every other block member: its size is the log's length.
+// RaftDev.state = 1: init received (the node-id promise is delivered).  Handlers run one at a time in dequeue order.
+__device__ __forceinline__ Rec rw_msg(const RaftCtx& c, uint32_t dest, uint32_t type, uint32_t p0) {
+  Rec m;                                                                          // send! (node.clj:110-115): no msg_id
+  m.round = 0; m.ticket = 0; m.idx = 0;
+  m.src = c.e; m.dest = dest; m.msg_id = 0; m.in_reply_to = 0;
+  m.tf = type; m.p0 = p0; m.p1 = 0;
+  return m;
+}
+
+// the replication thread (:104-114): (Thread/sleep 100) then replicate-step!, from process start, at the start of the
+// node's step.  The node's step may come after several periods (it is only stepped when due with a non-empty log, or
+// for mail): a period that passed with an empty log sent nothing, so the schedule moves on to the next period after now
+__device__ void rw_task(RaftCtx& c) {
+  const Params& p = c.p;
+  int64_t& next = p.gs_next_fire[c.e];
+  if (c.now < next) return;
+  const uint32_t n = p.rw_len[c.e];
+  if (n) rf_emit(c, rw_msg(c, c.gbase == c.e ? c.e + 1u : c.gbase, MS_T_REPLICATE, n));   // the lowest other member
+  const int64_t period = (int64_t)p.gs_interval_ms * kTickNs;
+  next += ((c.now - next) / period + 1) * period;
+}
+
+__device__ void rw_handle(RaftCtx& c, const Rec& m) {
+  const Params& p = c.p;
+  const uint32_t type = m.tf & 0xFFFFu, flags = m.tf >> 16;
+  if (flags & MS_F_REPLY) return;                                                 // handle-reply!: no rpcs (node.clj:131-139)
+  if (type != MS_T_INIT && !c.r->state) return;                                   // blocked on the node-id promise
+  if (type == MS_T_REPLICATE_ACK) return;                                         // nil timestamps: nothing to remove
+  const bool has_id = (flags & MS_F_MSG_ID) != 0;
+  Rec a;                                                                          // reply! (node.clj:116-119)
+  a.round = 0; a.ticket = 0; a.idx = 0;
+  a.src = c.e; a.dest = m.src; a.msg_id = 0;
+  a.in_reply_to = has_id ? m.msg_id : 0u;                                         // in_reply_to: nil without a msg_id
+  a.p0 = 0; a.p1 = 0;
+  uint64_t& lamport = p.rw_lamport[c.e];
+  uint32_t out_type = MS_T_ERROR;
+  if (type == MS_T_INIT) {                                                        // handle-init! (node.clj:141-151)
+    c.r->state = 1;
+    out_type = MS_T_INIT_OK;
+  } else if (type == MS_T_TXN) {                                                  // txn_rw_register_hat.clj:116-125
+    const uint32_t len = p.rw_len[c.e];
+    for (int i = 0; i < 4; i++) {
+      const uint32_t op = (uint32_t)(m.p1 >> (16 * i)) & 0xFFFFu;
+      if ((op >> 15) && (op & 0x3FFFu) >= p.rw_keys) { latch_error(c.st, E_VALUE_RANGE, op & 0x3FFFu); return; }
+    }
+    if (len >= p.rw_cap) { latch_error(c.st, E_TXN_RW_CAPACITY, c.e); return; }
+    const uint64_t ts = lamport++;                                                // apply-txn+: [lamport node-id]
+    ms_txn_rw_entry en;
+    en.lamport = ts; en.ops = m.p1; en.base = m.p0; en.pad = 0;
+    uint32_t* val = p.rw_val + (size_t)c.e * p.rw_keys;
+    uint64_t* wts = p.rw_ts + (size_t)c.e * p.rw_keys;
+    for (int i = 0; i < 4; i++) {
+      const uint32_t op = (uint32_t)(m.p1 >> (16 * i)) & 0xFFFFu, k = op & 0x3FFFu;
+      en.reads[i] = 0;
+      if (!(op >> 15)) continue;
+      if (op & (1u << 14)) { val[k] = m.p0 + (uint32_t)i; wts[k] = ts; }          // a fresh ts is above every stored one
+      else en.reads[i] = val[k];
+    }
+    p.rw_log[(size_t)c.e * p.rw_cap + len] = en;
+    p.rw_len[c.e] = len + 1u;                                                     // later-replicate!
+    out_type = MS_T_TXN_OK;
+    a.p0 = len; a.p1 = ts;
+  } else if (type == MS_T_REPLICATE) {                                            // :127-145
+    lamport += m.p0;                                                              // an empty txn per txn+
+    for (uint32_t n = c.gbase; n < c.gbase + c.gn; n++)
+      if (n != c.e) rf_emit(c, rw_msg(c, n, MS_T_REPLICATE_ACK, m.p0));           // other-node-ids, block order
+    return;
+  } else {
+    a.p0 = 10;                                                                    // "Unknown request type" (node.clj:155-163)
+  }
+  a.tf = out_type | ((has_id ? (uint32_t)MS_F_REPLY : 0u) << 16);
+  rf_emit(c, a);
+}
+
 // ------------------------------------------------------------------ txn-list-append on a persistent hash tree
 // demo/ruby/datomic_list_append.rb.  The database is a tree of immutable nodes stored in lww-kv under
 // unique pointers; lin-kv holds the pointer to the root (key "root" = key 0 here).  A txn (:340-353, under

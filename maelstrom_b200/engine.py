@@ -9,7 +9,7 @@ from . import _lib
 from ._lib import Body, Config, EVENT_DTYPE, JBODY_DTYPE, MSG_DTYPE, OP_DTYPE  # noqa: F401
 
 WORKLOADS = {"echo": 0, "broadcast": 1, "g-set": 2, "lin-kv": 3, "txn-list-append": 4, "txn-list-append-tree": 5,
-             "lin-kv-proxy": 6, "kafka": 7, "g-counter": 8, "pn-counter": 9}
+             "lin-kv-proxy": 6, "kafka": 7, "g-counter": 8, "pn-counter": 9, "txn-rw-register": 10}
 TOPOLOGIES = {"grid": 0, "line": 1, "total": 2, "tree": 3, "tree2": 3, "tree3": 4, "tree4": 5}
 DISTS = {"constant": 0, "uniform": 1, "exponential": 2}
 KIND_SERVER, KIND_CLIENT, KIND_HOST, KIND_SIM_CLIENT, KIND_SERVICE = 0, 1, 2, 3, 4
@@ -24,6 +24,8 @@ KAFKA_TYPES = dict(send=70, send_ok=71, poll=72, poll_ok=73, commit_offsets=74, 
                    list_committed_offsets=76, list_committed_offsets_ok=77)
 # the counter workloads' merge / merge_ok (MS_T_MERGE ...): the device's own encoding, as kafka's
 COUNTER_TYPES = dict(merge=80, merge_ok=81)
+# the txn-rw-register node's replicate / replicate_ack (MS_T_REPLICATE ...): the device's own encoding, as kafka's
+TXN_RW_TYPES = dict(replicate=90, replicate_ack=91)
 TYPE_NAMES = {v: k for k, v in TYPES.items()}
 F_MSG_ID, F_REPLY, F_CREATE, F_APPENDS = 1, 2, 4, 8
 RECV_BIT = 1 << 63
@@ -37,7 +39,7 @@ class SimError(RuntimeError):
 
 def body(type, msg_id=None, in_reply_to=None, p0=0, p1=0, create=False, appends=False):
     b = Body()
-    b.type = {**TYPES, **KAFKA_TYPES, **COUNTER_TYPES}[type] if isinstance(type, str) else type
+    b.type = {**TYPES, **KAFKA_TYPES, **COUNTER_TYPES, **TXN_RW_TYPES}[type] if isinstance(type, str) else type
     b.flags = ((F_MSG_ID if msg_id is not None else 0) | (F_REPLY if in_reply_to is not None else 0) |
                (F_CREATE if create else 0) | (F_APPENDS if appends else 0))
     b.msg_id = msg_id or 0
@@ -101,7 +103,7 @@ class Sim:
         # named spellings of ms_config.reserved[]
         for name, slot in (("history_rounds", 0), ("use_graph", 1), ("n_keys", 2), ("raft_log_cap", 3),
                            ("raft_group", 4), ("rpc_table", 5), ("tree_ptrs", 3), ("tree_cache", 4),
-                           ("kafka_keys", 2), ("kafka_log_cap", 3)):
+                           ("kafka_keys", 2), ("kafka_log_cap", 3), ("txn_rw_keys", 2), ("txn_rw_log_cap", 3)):
             if name in sizing:
                 cfg.reserved[slot] = int(sizing.pop(name))
         for k, v in sizing.items():
@@ -225,6 +227,43 @@ class Sim:
         out = np.zeros(n, dtype=np.int64)
         self._chk(self.L.ms_counter_state(self.h, node, out.ctypes.data, n))
         return out[:n // 2], out[n // 2:]
+
+    def add_txn_rw_clients(self, n_clients, interval_ns, time_limit_ns, key_period_ns, key_count=1, min_len=1, max_len=4,
+                           timeout_ns=0, first_name=0):
+        """ms_add_txn_rw_clients: closed-loop txn-rw-register clients on the device (client k on server k mod n_nodes);
+        returns the first endpoint index.  txn_rw_history() returns their records"""
+        rc = _lib.TxnRwGenConfig(n_clients, min_len, max_len, key_count, interval_ns, timeout_ns, time_limit_ns,
+                                 key_period_ns)
+        return self._chk(self.L.ms_add_txn_rw_clients(self.h, C.byref(rc), first_name))
+
+    def txn_rw_history(self, cap=1 << 20):
+        """ms_txn_rw_history_drain: the txn-rw-register clients' records since the last call, in (time, round, client)
+        order"""
+        parts = []
+        while True:
+            out = np.zeros(cap, dtype=_lib.TXN_RW_HIST_DTYPE)
+            n = C.c_size_t(0)
+            self._chk(self.L.ms_txn_rw_history_drain(self.h, out.ctypes.data, cap, C.byref(n)))
+            parts.append(out[:n.value])
+            if n.value < cap:
+                break
+        return np.concatenate(parts)
+
+    def txn_rw_log(self, node):
+        """ms_txn_rw_log: node's completed txns in log order (TXN_RW_ENTRY_DTYPE)"""
+        n = self._chk(self.L.ms_txn_rw_log(self.h, node, None, 0))
+        out = np.zeros(n, dtype=_lib.TXN_RW_ENTRY_DTYPE)
+        self._chk(self.L.ms_txn_rw_log(self.h, node, out.ctypes.data, n))
+        return out
+
+    def txn_rw_state(self, node):
+        """ms_txn_rw_state: (lamport, log length, values, timestamps) of node; values[k] = 0 is nil, ts[k] the lamport
+        of the write"""
+        lamport, n = C.c_uint64(0), C.c_uint32(0)
+        k = self._chk(self.L.ms_txn_rw_state(self.h, node, None, None, None, None, 0))
+        val, ts = np.zeros(k, dtype=np.uint32), np.zeros(k, dtype=np.uint64)
+        self._chk(self.L.ms_txn_rw_state(self.h, node, C.byref(lamport), C.byref(n), val.ctypes.data, ts.ctypes.data, k))
+        return lamport.value, n.value, val, ts
 
     def history(self, cap=1 << 20):
         """ms_history_drain: the history records since the last call, in (time, round, client) order"""
@@ -488,6 +527,7 @@ HIST_TYPES = ("invoke", "ok", "fail", "info")              # MS_H_*
 HF_KV_READ, HF_KV_WRITE, HF_KV_CAS = 2, 3, 4              # MS_HF_KV_*
 HF_KAFKA_SEND, HF_KAFKA_POLL, HF_KAFKA_ASSIGN, HF_KAFKA_CRASH = 10, 11, 12, 13   # MS_HF_KAFKA_*
 HF_COUNTER_ADD = 14                                       # MS_HF_COUNTER_ADD
+HF_TXN_RW = 15                                            # MS_HF_TXN_RW
 H_NEMESIS = 0xFFFFFFFF                                    # MS_H_NEMESIS: the client of a nemesis record
 HF_NEM_ONE, HF_NEM_MAJORITY, HF_NEM_MINORITY_THIRD, HF_NEM_STOP = 5, 6, 7, 8   # MS_HF_NEM_*
 HF_NEM_MAJORITIES_RING = 9                                # MS_HF_NEM_MAJORITIES_RING

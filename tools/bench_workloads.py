@@ -347,9 +347,59 @@ def bench_pn_counter(mb, n, group, clients_per_node, steps, step_ms=200, interva
                 msgs_per_op=msgs / int(tally[0]) if tally[0] else None, card=card())
 
 
+def bench_txn_rw(mb, n, group, clients_per_node, steps, step_ms=200, interval_ms=100, key_count=4):
+    """The GPU scale shape of tests/test_txn_rw.py: n txn-rw-register nodes (demo/clojure/txn_rw_register_hat.clj) in
+    blocks of `group`, replicating every 100 ms, with clients_per_node closed-loop txn clients per node
+    (ms_add_txn_rw_clients, 1 to 4 micro-ops, key_count keys at a time).  The history is drained after every step;
+    device time is the engine's CUDA-event timer around each step's rounds."""
+    from maelstrom_b200.engine import KIND_SIM_CLIENT, OP_DTYPE, TYPES, F_MSG_ID
+    n_clients = n * clients_per_node
+    cap = 2 * (steps + 2) * step_ms * clients_per_node // interval_ms + 64   # ~2 txns a client per interval at most
+    sim = mb.Sim(n, workload="txn-rw-register", raft_group=group, txn_rw_log_cap=cap, latency_dist="constant",
+                 latency_mean_ms=0, journal_level=0, max_endpoints=n + n_clients + 8, ring_cap=64, max_window=64,
+                 server_ring_cap=64, server_max_window=32)
+    c = sim.add_endpoint("c%d" % (1 << 30), KIND_SIM_CLIENT)
+    rows = ops_array(n, OP_DTYPE)
+    rows["src"], rows["dest"] = c, np.arange(n)
+    rows["body"]["type"], rows["body"]["flags"], rows["body"]["msg_id"] = TYPES["init"], F_MSG_ID, np.arange(n) + 1
+    rows["time_ns"] = (np.arange(n) % 128) * 1_000_000       # 32 init_ok a millisecond fit the sink's ring
+    rows = rows[np.argsort(rows["time_ns"], kind="stable")]
+    sim.schedule(rows)
+    sim.run(step_ms * 1_000_000)
+    sim.add_txn_rw_clients(n_clients, interval_ns=interval_ms * 1_000_000, time_limit_ns=1 << 62,
+                           key_period_ns=500 * 1_000_000, key_count=key_count)
+    tally = np.zeros(4, dtype=np.int64)                # invoke / ok / fail / info
+    dev_ms = wall = 0.0
+    m0 = r0 = 0
+    for k in range(steps + 1):                         # step 0 is the warm-up: not timed, not counted
+        now_ms = (k + 1) * step_ms
+        t0 = time.time()
+        sim.timer_begin()
+        sim.run((now_ms + step_ms) * 1_000_000)
+        ms = sim.timer_end()                           # ends in a synchronise on the event
+        h = sim.txn_rw_history()
+        dt = time.time() - t0
+        if k == 0:
+            m0, r0 = sim.stats()["all"]["msg-count"], sim.counters()["recvs"]
+            continue
+        dev_ms += ms
+        wall += dt
+        tally += np.bincount(h["type"], minlength=4)[:4]
+    msgs = sim.stats()["all"]["msg-count"] - m0
+    recvs = sim.counters()["recvs"] - r0
+    done = int(tally[1:].sum())
+    return dict(workload="txn-rw-register nodes, closed-loop txn clients on the device", nodes=n, group=group,
+                clients=n_clients, virtual_ms=steps * step_ms, client_interval_ms=interval_ms, replicate_ms=100,
+                key_count=key_count, latency="constant 0 ms", device_ms=dev_ms, wall_s=wall,
+                rounds=sim.counters()["rounds"], ops_invoked=int(tally[0]), ops_completed=done, ok=int(tally[1]),
+                fail=int(tally[2]), info=int(tally[3]), ops_per_s_wall=done / wall if wall > 0 else None,
+                msgs_per_s=recvs / (dev_ms / 1e3) if dev_ms > 0 else None,
+                msgs_per_op=msgs / int(tally[0]) if tally[0] else None, card=card())
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--only", default="", help="run one case: g-set, services, txn, raft, kv-clients, kv-proxy, kafka or pn-counter")
+    ap.add_argument("--only", default="", help="run one case: g-set, services, txn, raft, kv-clients, kv-proxy, kafka, pn-counter or txn-rw-register")
     ap.add_argument("--emul", action="store_true", help="run on the CPU SIMT emulator (script check only)")
     ap.add_argument("--tiny", action="store_true")
     a = ap.parse_args()
@@ -364,13 +414,15 @@ def main():
             runs = {"g-set": lambda: bench_gset(mb, 12, 8, 512, 10, 4), "services": lambda: bench_services(mb, 40, 5),
                     "txn": lambda: bench_txn(mb, 3, 12, 5), "raft": lambda: bench_raft(mb, 3, 4260, 2),
                     "kv-clients": lambda: bench_kv_clients(mb, 11, 5, 3), "kv-proxy": lambda: bench_kv_proxy(mb, 15, 5, 3),
-                    "kafka": lambda: bench_kafka(mb, 16, 4, 4, 3), "pn-counter": lambda: bench_pn_counter(mb, 15, 5, 2, 3)}
+                    "kafka": lambda: bench_kafka(mb, 16, 4, 4, 3), "pn-counter": lambda: bench_pn_counter(mb, 15, 5, 2, 3),
+                    "txn-rw-register": lambda: bench_txn_rw(mb, 16, 2, 2, 3)}
         else:
             runs = {"g-set": lambda: bench_gset(mb, 1024, 100, 1 << 14, 200, 64), "services": lambda: bench_services(mb, 1 << 14, 20),
                     "txn": lambda: bench_txn(mb, 256, 1 << 11, 20), "raft": lambda: bench_raft(mb, 5, 10_000, 4),
                     "kv-clients": lambda: bench_kv_clients(mb, 65536, 5, 12), "kv-proxy": lambda: bench_kv_proxy(mb, 4095, 5, 15),
                     "kafka": lambda: bench_kafka(mb, 4096, 4, 4, 15),
-                    "pn-counter": lambda: bench_pn_counter(mb, 4095, 5, 4, 15)}
+                    "pn-counter": lambda: bench_pn_counter(mb, 4095, 5, 4, 15),
+                    "txn-rw-register": lambda: bench_txn_rw(mb, 4096, 2, 4, 15)}
         for name, r in runs.items():
             if not a.only or a.only == name:
                 print(json.dumps(r(), sort_keys=True), flush=True)
